@@ -11,15 +11,20 @@ val.py:378-383).  Metric: images/s.
              written as the compact records the post-process reads (checked equal to Model.forward + NMS before timing)
   e2e        the same step through the public API from PINNED HOST memory: H2D of the uint8 batch and D2H
              of the detections inside the timed region
-  roofline   conv_tc_kernel (tcgen05 implicit GEMM), the dominant kernel: algorithmic conv FLOPs per launch
+  roofline   conv_wgmma_kernel (wgmma implicit GEMM), the dominant kernel: algorithmic conv FLOPs per launch
              / mean launch duration measured with CUDA events around every launch in the timed steps,
-             against MEASURED_PEAKS.json's burst bf16 figure (frac) and its sustained one (frac_sustained)
+             against MEASURED_PEAKS.json's burst bf16 figure (frac) and its sustained one (frac_sustained) when that file
+             exists, else against the H100 SXM data sheet (dense bf16, 700 W)
   parity     the benchmarked plan checked against the fp32 oracle before anything is timed (bf16-noise-floor rule), and the
              fused Detect-records plan checked equal to Model.forward + non_max_suppression_obb
   nms        the other half of the metric: rotated-NMS boxes/s and pair-IoUs/s, 1k-200k candidates, beside the reference's own
              CUDA kernel K1 on the same GPU and its CPU kernel
-  extra.eager_torch_b200   the reference's GPU path restated with eager PyTorch/cuDNN fp16 + K1 on this GPU (the bar, not the target);
-  train.eager_torch_b200   the same for the training step (autocast + GradScaler + SGD)
+  extra.eager_torch   the reference's GPU path restated with eager PyTorch/cuDNN fp16 + K1 on this GPU (the bar, not the target);
+  train.eager_torch   the same for the training step (autocast + GradScaler + SGD)
+  --dump-outputs DIR   after the timed inference steps, the last step's detections as DIR/detections.npy (float32
+             [B, max_det, 7], rows past an image's count zeroed) and DIR/counts.npy (float64 [B]); the inputs are seeded, so
+             two builds can be compared output for output.  Only the inference path is dumped: nothing of the train leg
+             (loss, loss items, updated parameters) is written
   cpu_baseline   the oracle port (fp32 torch restatement of the reference's eager CPU path + the reference's
              own CPU NMS kernel from oracle/_ref when present) on the host cores, bounded sample
 
@@ -65,28 +70,30 @@ def parse():
     ap.add_argument("--train-batch", type=int, default=TRAIN_BATCH)
     ap.add_argument("--train-steps", type=int, default=10)
     ap.add_argument("--no-nms-sweep", action="store_true", help="skip the rotated-NMS boxes/s sweep (the `nms` object)")
-    ap.add_argument("--no-eager", action="store_true", help="skip the eager-PyTorch-on-this-GPU bar (`extra.eager_torch_b200`)")
+    ap.add_argument("--no-eager", action="store_true", help="skip the eager-PyTorch-on-this-GPU bar (`extra.eager_torch`)")
     ap.add_argument("--no-extra-models", action="store_true", help="skip the yolov5m b16 inference line (`extra.yolov5m_b16_inference`)")
     ap.add_argument("--no-parity-gate", action="store_true", help="skip the engine-vs-oracle check of the benchmarked plan")
     ap.add_argument("--slots", type=int, default=2, help="batches in flight per GPU, one stream + one plan each (DetectPipeline slots)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's detections (and per-image counts) as .npy files under DIR")
     return ap.parse_args()
 
 
 def peaks():
-    """MEASURED_PEAKS.json (driver-written): HBM copy bandwidth and cuBLAS bf16 throughput, burst and sustained.  The conv
-    launches are timed one by one with CUDA events inside a region of a few tens of milliseconds at the full 1965 MHz clock
-    (no power capping, see `clocks`), so the BURST figure is the denominator of roofline.frac; the sustained one is reported
-    beside it (frac_sustained) and is the denominator of the multi-second train leg."""
+    """MEASURED_PEAKS.json (written per machine, not part of the repository): HBM copy bandwidth and cuBLAS bf16 throughput,
+    burst and sustained.  The conv launches are timed one by one with CUDA events inside a region of a few tens of
+    milliseconds, so the BURST figure is the denominator of roofline.frac; the sustained one is reported beside it
+    (frac_sustained) and is the denominator of the multi-second train leg.  Without the file: the H100 SXM data sheet."""
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return dict(tflops=float(d.get("bf16_tflops", 1590.0)), tflops_sustained=float(d.get("bf16_tflops_sustained", 1400.0)),
-                    hbm=float(d.get("hbm_gbs", 6650.0)), src="measured (MEASURED_PEAKS.json: burst bf16 for frac, sustained for frac_sustained)")
-    return dict(tflops=1590.0, tflops_sustained=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+        return dict(tflops=float(d.get("bf16_tflops", 989.0)), tflops_sustained=float(d.get("bf16_tflops_sustained", 989.0)),
+                    hbm=float(d.get("hbm_gbs", 3350.0)), src="measured (MEASURED_PEAKS.json: burst bf16 for frac, sustained for frac_sustained)")
+    return dict(tflops=989.0, tflops_sustained=989.0, hbm=3350.0, src="H100 SXM data sheet (dense bf16, HBM3; 700 W card)")
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md's clocks line), through NVML
+    """SM clock and throttle reasons sampled DURING the timed region, through NVML
     (nvidia_ml_py) from a thread every 20 ms; nvidia-smi's own polling loop takes longer to start than a short run lasts."""
 
     def __init__(self, index):
@@ -171,7 +178,7 @@ def cpu_arm(size, batch, steps, warmup, budget_s=25.0, use_ref_nms=False):
     x8 = synth_batch(b, 0)
     kind = "port"
     nms_note = "C++ oracle rotated NMS (1 thread)"
-    if use_ref_nms:  # the reference's own nms_rotated_cpu kernel, compiled from /root/reference into oracle/_ref
+    if use_ref_nms:  # the reference's own nms_rotated_cpu kernel, compiled by oracle/build_ref.py into oracle/_ref
         try:
             import oracle.postprocess as pp
             from oracle.build_ref import load_ref
@@ -256,7 +263,7 @@ def workload_config(args):
             "in_flight": f"our arm: {getattr(args, 'slots', 1)} batches per GPU, each on its own stream with its own plan (DetectPipeline "
                          "slots); ms_per_step = timed region / steps (throughput time, not the latency of one batch: see "
                          "single_stream).  The reference arm processes one batch at a time",
-            "l2": "per-step working set (activations > 3 GB) exceeds the 126 MB L2; no explicit flush"}
+            "l2": "per-step working set (activations > 3 GB) exceeds the 50 MB L2; no explicit flush"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -430,7 +437,7 @@ def nms_sweep(dev, seeds=(0, 1, 2), cpu_budget_s=25.0):
     ("sparse": nothing suppressed, worst case for the pair count), unique scores, thr 0.4.  Per (layout, N), median over
     the seeds:  ours through the reference-facing op nms_rotated(dets, scores, thr) on class-OFFSET boxes (the reference's
     own mode, general.py:849-851) and through the segmented op on raw boxes; the reference's CUDA kernel K1
-    (nms_rotated_cuda.cu compiled from /root/reference into oracle/_ref) on the same GPU and inputs, keep lists compared;
+    (nms_rotated_cuda.cu compiled by oracle/build_ref.py into oracle/_ref) on the same GPU and inputs, keep lists compared;
     the reference's CPU kernel for the sizes a time budget allows."""
     import ctypes
     import numpy as np
@@ -620,6 +627,20 @@ def eager_torch_arm(model_cpu, x_u8_dev, steps, warmup):
 # ------------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, dets, B):
+    """The last timed step's result as the pipeline hands it to a caller: packed detections [B, max_det, 7] and the rows per
+    image.  Rows past an image's count are not part of the result and are written as zeros."""
+    import numpy as np
+    out7 = dets[0].float().cpu().numpy().copy()
+    counts = np.asarray(dets[1].tolist()[:B], dtype=np.int64)
+    for b in range(B):
+        out7[b, counts[b]:] = 0.0
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "detections.npy", out7.astype(np.float32))
+    np.save(d / "counts.npy", counts.astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -736,6 +757,8 @@ def run_ours(args):
     pipe.join()
     ms_total, dets = timed(step_device, args.steps, pipe)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dets, B)
     for dd in last.values():                     # the last batch of every slot
         rows = dd[1].tolist()
         if rows[B] > dd[2] or min(rows) < 0:
@@ -807,14 +830,9 @@ def run_ours(args):
     conv_ms = [sum(evs[s][i][0].elapsed_time(evs[s][i][1]) for s in range(steps_r)) / steps_r for i in range(n_conv)]
     tot_conv_ms = sum(conv_ms)
     ach_tflops = sum(conv_flops) / (tot_conv_ms / 1e3) / 1e12
-    traffic, traffic_src = None, None
-    tp = ROOT / "profiles" / "r2_conv_traffic.json"   # dram__bytes_read+write per launch from one `ncu --set full` capture
-    if tp.exists() and args.model == MODEL and B == BATCH:
-        tj = json.loads(tp.read_text())
-        traffic, traffic_src = tj["dram_bytes_per_launch_mean"], tj["source"]
-    roof = {"bound": "tensor", "kernel": "conv_tc_kernel", "achieved": ach_tflops, "peak": pk["tflops"],
+    roof = {"bound": "tensor", "kernel": "conv_wgmma_kernel", "achieved": ach_tflops, "peak": pk["tflops"],
             "unit": "TFLOP/s", "frac": ach_tflops / pk["tflops"], "frac_sustained": ach_tflops / pk["tflops_sustained"],
-            "peak_sustained": pk["tflops_sustained"], "traffic": traffic, "traffic_source": traffic_src,
+            "peak_sustained": pk["tflops_sustained"],
             "algorithmic_bytes_per_launch": eng.hbm_bytes / n_conv, "peak_source": pk["src"],
             "launches_per_step": n_conv, "flops_per_launch": sum(conv_flops) / n_conv,
             "mean_launch_us": tot_conv_ms / n_conv * 1e3, "conv_share_of_step": tot_conv_ms / ms_single,
@@ -885,7 +903,7 @@ def run_ours(args):
                        "batch i-slots while the later ones compute)"},
         "single_stream": {"ms_per_step": ms_single, "value": world * B / (ms_single / 1e3), "unit": "images/s",
                           "what": "the same device-resident step with ONE batch in flight on one stream"},
-        "gpu_launches": (1 + len(eng.ops) + 25) * args.steps,  # layout pass + conv / pool launches + the post-process kernels (profiles/r2_launches_infer.csv: 79 per step)
+        "gpu_launches": (1 + len(eng.ops) + 25) * args.steps,  # layout pass + conv / pool launches + the post-process kernels
         "detections_per_image": det_per_img, "step_breakdown": breakdown,
         "clocks": clocks, "roofline": roof,
     }
@@ -896,7 +914,7 @@ def run_ours(args):
     if eager is not None or extra_m is not None:
         line["extra"] = {}
         if eager is not None:
-            line["extra"]["eager_torch_b200"] = eager
+            line["extra"]["eager_torch"] = eager
         if extra_m is not None:
             line["extra"]["yolov5m_b16_inference"] = extra_m
     if not args.no_cpu_baseline and world == 1:
@@ -906,9 +924,9 @@ def run_ours(args):
         line["train"] = train
         if world == 1 and not args.no_eager:
             try:
-                train["eager_torch_b200"] = eager_train_arm(args.train_model, dev, train.get("global_batch", 8))
+                train["eager_torch"] = eager_train_arm(args.train_model, dev, train.get("global_batch", 8))
             except Exception as e:  # pragma: no cover
-                train["eager_torch_b200"] = {"unavailable": f"{type(e).__name__}: {e}"}
+                train["eager_torch"] = {"unavailable": f"{type(e).__name__}: {e}"}
             torch.cuda.empty_cache()
         if not args.no_cpu_baseline and world == 1:
             tb = cpu_train_arm(args.train_model)

@@ -1,11 +1,11 @@
-/* y5obb.h — C ABI of the B200-native yolov5_obb hot path (liby5obb.so).
+/* y5obb.h — C ABI of the H100-native (sm_90a) yolov5_obb hot path (liby5obb.so).
  *
  * Plain pointers and sizes only; every pointer is a DEVICE pointer unless its name ends in _host.
  * All entry points are asynchronous on `stream` (a cudaStream_t passed as void*) unless stated, never
  * call cudaDeviceSynchronize, and return 0 on success or a Y5OBB_E* code (the Python shims raise
  * RuntimeError on != 0, as the reference's AT_ASSERTM / AT_CUDA_CHECK do).
  *
- * Each declaration cites the reference interface it replaces (paths relative to /root/reference).
+ * Each declaration cites the reference interface it replaces (paths relative to the yolov5_obb source tree).
  */
 #ifndef Y5OBB_H_
 #define Y5OBB_H_
@@ -21,12 +21,12 @@ extern "C" {
 #define Y5OBB_EINVAL 1     /* bad argument (null pointer, negative size, unsupported shape) */
 #define Y5OBB_EWORKSPACE 2 /* workspace too small: call the matching *_workspace_bytes */
 #define Y5OBB_ECUDA 3      /* a CUDA call failed; y5obb_last_cuda_error() has the cudaError_t */
-#define Y5OBB_EARCH 4      /* device is not sm_100 */
+#define Y5OBB_EARCH 4      /* device is not sm_90 */
 
 /* ---- library ------------------------------------------------------------------------------- */
 int y5obb_abi_version(void);            /* bumps when a signature changes */
 int y5obb_last_cuda_error(void);        /* cudaError_t of the last failing CUDA call on this thread */
-const char* y5obb_build_info(void);     /* "sm_100a nvcc <ver> <date>" */
+const char* y5obb_build_info(void);     /* "liby5obb sm_90a <date> <time>" */
 
 /* ---- rotated NMS ---------------------------------------------------------------------------
  * Replaces  utils/nms_rotated/src/nms_rotated_ext.cpp:25-39  (nms_rotated(dets, scores, thr))
@@ -98,7 +98,7 @@ int y5obb_nms_obb_f32(const float* pred, int64_t batch, int64_t anchors, int no,
                       void* workspace, size_t workspace_bytes, void* stream);
 
 
-/* ---- convolution (tcgen05 implicit GEMM) ---------------------------------------------------
+/* ---- convolution (wgmma implicit GEMM) -----------------------------------------------------
  * Replaces the cuDNN/ATen calls behind models/common.py:37-49 (Conv.forward_fuse = conv + folded-BN
  * bias + SiLU), :94-104 (Bottleneck residual), :267-274 (Concat, as a channel-offset store),
  * nn.Upsample(2x nearest) (models/yolov5*.yaml head) and models/yolo.py:49-81 (Detect).
@@ -120,14 +120,6 @@ typedef struct y5obb_conv y5obb_conv_t;
 #define Y5OBB_CONV_NO_PDL 32       /* flags: plain stream-ordered launch (default: programmatic dependent launch - the kernel's
                                       prologue overlaps the previous kernel's tail and it waits, griddepcontrol.wait, before its
                                       first global-memory access; also switched off by the environment variable Y5OBB_NO_PDL=1) */
-#define Y5OBB_CONV_MSUB1 128       /* flags: 128-pixel tiles only (default: up to four 128-pixel sub-tiles per tile) */
-#define Y5OBB_CONV_NO_UP_TMA 2048  /* flags: the 2x up-sampled copy through per-thread stores (default: four TMA stores of the staged tile) */
-#define Y5OBB_CONV_NO_DUAL 4096    /* flags: always one CTA per SM.  (Two CTAs per SM - 256 TMEM columns, half the shared memory and four
-                                      epilogue warps each - is an opt-in experiment, environment variable Y5OBB_DUAL; measured slower) */
-#define Y5OBB_CONV_NO_RES_RED 16384 /* flags: when `res` IS `out` (in-place Bottleneck add) the default adds the tile into memory with a TMA
-                                      reduce-add (bf16 add at L2: the sum is rounded twice); this flag keeps the epilogue's own fp32 add */
-#define Y5OBB_CONV_EPI2 8192       /* flags: reserved (two staging buffers per epilogue warp are the default; four: environment variable Y5OBB_EPI_BUFS=4, measured slower) */
-#define Y5OBB_CONV_ACC2 64         /* flags: two TMEM accumulator stages only (A-B comparison; default: as many as 512 columns hold) */
 
 typedef struct {
   const void* in;            /* bf16 NHWC slice */
@@ -169,13 +161,6 @@ int y5obb_conv_run(const y5obb_conv_t* conv, void* stream);
 int y5obb_conv_info(const y5obb_conv_t* conv, double* flops, double* hbm_bytes, int* grid, int* block_n,
                     int* block_k, int* stages);
 void y5obb_conv_destroy(y5obb_conv_t* conv);
-/* Profiling aid: CTA 0 of every later run writes clock64() stamps of its producer / MMA / epilogue roles for its first 32
- * tiles into dev_buf ([3][32][8] uint64, device memory; NULL switches it off).  Results are unaffected. */
-int y5obb_conv_debug_timestamps(y5obb_conv_t* conv, unsigned long long* dev_buf);
-/* Profiling aid: resident CTAs per SM the runtime grants the one-CTA (dual = 0, 320 threads) or two-CTA (dual = 1, 192 threads)
- * instantiation of the kernel for a given dynamic shared-memory size, with its register count and static shared memory. */
-int y5obb_conv_debug_occupancy(int dual, int threads, size_t dyn_smem, int* blocks_per_sm, int* regs, int* static_smem);
-int y5obb_wgrad_debug_occupancy(size_t dyn_smem, int* blocks_per_sm, int* regs);
 
 /* ---- HBM-bound helpers around the conv stack -------------------------------------------------
  * y5obb_stem_s2d: NCHW fp32 image [B,3,H,W] -> 2x2 space-to-depth NHWC bf16 [B,H/2,W/2,16] (channel
@@ -269,7 +254,7 @@ int y5obb_bn_silu_bwd(const void* z, int64_t z_pix_stride, const void* dy, int64
                       float* sum_du, float* sum_dux, void* dz, int64_t dz_pix_stride, void* gres,
                       int64_t gres_pix_stride, int gres_accumulate, float* dgamma, float* dbeta, int param_accumulate,
                       float* scratch, int64_t scratch_floats, void* stream);
-/* ---- weight gradient (tcgen05 GEMM over the pixel axis) -------------------------------------------
+/* ---- weight gradient (wgmma GEMM over the pixel axis) ---------------------------------------------
  * dW[tap][co][ci] (fp32, ACCUMULATED with atomics: zero it first) = sum_{b,ho,wo} dz[b,ho,wo,co] * x[b,s*ho+kh-ph,s*wo+kw-pw,ci].
  * Replaces the cuDNN wgrad autograd calls for models/common.py:37-46 under train.py:333.  Operands are the NHWC bf16
  * gradient / activation buffers themselves (channel slices allowed: pix strides in elements, multiples of 8; rows and

@@ -1,7 +1,7 @@
 // y5obb_devkit.hpp - the DOTA devkit's GPU entry points, exported by liby5obb.so under the reference's own C++ names, so that
 // DOTA_devkit/poly_nms_gpu/poly_nms.pyx and poly_overlaps.pyx link against liby5obb.so instead of poly_nms_kernel.cu /
 // poly_overlaps_kernel.cu with no source change (`cdef extern from "poly_nms.hpp"` -> this header).
-// Replaces /root/reference/DOTA_devkit/poly_nms_gpu/poly_nms.hpp:9-10 and poly_overlaps.hpp:1.  Host pointers in and out,
+// Replaces DOTA_devkit/poly_nms_gpu/poly_nms.hpp:9-10 and poly_overlaps.hpp:1.  Host pointers in and out,
 // synchronous on the default stream of `device_id`; CUDA errors are printed to stdout, not returned (poly_nms_kernel.cu:20-27).
 #ifndef Y5OBB_DEVKIT_HPP_
 #define Y5OBB_DEVKIT_HPP_

@@ -6,7 +6,7 @@ the product package.  This is "the bar to beat" of SURVEY §2.3 L1: what `val.py
     NCHW (the reference never sets channels_last);
   * Detect exactly as models/yolo.py:49-81 (oracle.model_ref.detect_fwd);
   * non_max_suppression_obb (utils/general.py:772-862) as the per-image Python loop over the reference's own CUDA kernel K1
-    (utils/nms_rotated/src/nms_rotated_cuda.cu compiled from /root/reference into oracle/_ref).
+    (utils/nms_rotated/src/nms_rotated_cuda.cu compiled by oracle/build_ref.py into oracle/_ref).
 """
 import torch
 import torch.nn.functional as F

@@ -1,7 +1,7 @@
 """fp32 PyTorch restatement of the reference loss — TEST INFRASTRUCTURE (never imported by the product).
 
-Follows /root/reference/utils/loss.py:93-120 (ComputeLoss.__init__), :122-192 (__call__), :194-275
-(build_targets) and /root/reference/utils/metrics.py:201-243 (bbox_iou, CIoU branch), with the one source shim
+Follows utils/loss.py:93-120 (ComputeLoss.__init__), :122-192 (__call__), :194-275
+(build_targets) and utils/metrics.py:201-243 (bbox_iou, CIoU branch), with the one source shim
 SURVEY §8(c) lists (clamp bound as int).  Gradients come from torch autograd.  Pinned by
 tests/golden/loss_golden.npz = outputs of the REFERENCE ComputeLoss on seeded inputs.
 """

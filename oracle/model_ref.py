@@ -1,8 +1,8 @@
 """fp32 PyTorch restatement of the reference forward pass — TEST INFRASTRUCTURE (torch fp32 reference
 for a floating-point kernel; never imported by the product package).
 
-Follows /root/reference/models/common.py:37-49 (Conv), :94-104 (Bottleneck), :126-138 (C3), :181-196
-(SPPF), :267-274 (Concat), nn.Upsample, /root/reference/models/yolo.py:49-81 (Detect) and :163-181
+Follows models/common.py:37-49 (Conv), :94-104 (Bottleneck), :126-138 (C3), :181-196
+(SPPF), :267-274 (Concat), nn.Upsample, models/yolo.py:49-81 (Detect) and :163-181
 (_forward_once), operating on the parameter containers of yolov5_obb_b200.yolo.Model (same names and
 shapes as the reference modules).  Pinned by tests/golden/model_golden.npz, which holds outputs of the
 REFERENCE model itself for the same seed (tests/golden/make_model_golden.py).

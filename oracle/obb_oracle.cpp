@@ -1,11 +1,11 @@
 // CPU oracle for the rotated-box path (TEST INFRASTRUCTURE — never linked into the product library).
 //
 // Restates, in scalar C++ with no FMA contraction (build with -ffp-contract=off), the algorithm of
-//   /root/reference/utils/nms_rotated/src/box_iou_rotated_utils.h:57-360   (single_box_iou_rotated)
-//   /root/reference/utils/nms_rotated/src/nms_rotated_cpu.cpp:8-61          (greedy NMS, suppress if IoU >= thr)
-//   /root/reference/utils/nms_rotated/src/nms_rotated_cuda.cu:12-134        (greedy NMS, suppress if IoU >  thr)
-//   /root/reference/utils/nms_rotated/nms_rotated_wrapper.py:6-46           (min(w,h) < 0.001 pre-filter)
-//   /root/reference/utils/general.py:772-862                                (non_max_suppression_obb)
+//   utils/nms_rotated/src/box_iou_rotated_utils.h:57-360   (single_box_iou_rotated)
+//   utils/nms_rotated/src/nms_rotated_cpu.cpp:8-61          (greedy NMS, suppress if IoU >= thr)
+//   utils/nms_rotated/src/nms_rotated_cuda.cu:12-134        (greedy NMS, suppress if IoU >  thr)
+//   utils/nms_rotated/nms_rotated_wrapper.py:6-46           (min(w,h) < 0.001 pre-filter)
+//   utils/general.py:772-862                                (non_max_suppression_obb)
 //
 // Two hull-ordering variants exist in the reference and both are restated here:
 //   variant 0 ("host"):   std::sort with the angle/distance comparator (box_iou_rotated_utils.h:221-233)
@@ -13,7 +13,7 @@
 // Variant 1 reproduces the device ORDER of operations but not nvcc's FMA contraction; the GPU tests
 // therefore compare IoU values against it with a tolerance and keep lists on inputs whose decisive
 // IoUs are not within that tolerance of the threshold; bit-for-bit device parity is checked against
-// oracle/_ref (the reference's own kernels compiled from /root/reference).
+// oracle/_ref (the reference's own kernels compiled by oracle/build_ref.py).
 //
 // Pinning: oracle/_ref/nms_rotated_ref (reference CPU extension built here) must agree with variant 0
 // bit for bit — tests/test_oracle_pin.py and the committed tests/golden/*.npz check exactly that.

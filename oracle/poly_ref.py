@@ -1,8 +1,8 @@
 """Polygon IoU and the tile-merge polygon NMS of the DOTA devkit — TEST INFRASTRUCTURE for SURVEY section 8f rank 4
 (never imported by the product package).
 
-Follows /root/reference/DOTA_devkit/polyiou.cpp:9-128 (iou_poly: the signed-triangle-fan intersection area of two
-quadrilaterals, eps = 1e-8 sign test) and /root/reference/DOTA_devkit/ResultMerge_multi_process.py:62-123
+Follows DOTA_devkit/polyiou.cpp:9-128 (iou_poly: the signed-triangle-fan intersection area of two
+quadrilaterals, eps = 1e-8 sign test) and DOTA_devkit/ResultMerge_multi_process.py:62-123
 (py_cpu_nms_poly_fast: greedy NMS in descending score with an axis-aligned pre-filter whose areas use the +1 pixel
 convention while the intersection does not).  Pinned against the reference's own polyiou.cpp compiled in place
 (oracle/_ref/libref_polyiou.so, oracle/build_ref.py) and tests/golden/poly_golden.npz."""

@@ -1,4 +1,4 @@
-"""CPU restatement of /root/reference/utils/general.py:772-862 (non_max_suppression_obb) —
+"""CPU restatement of utils/general.py:772-862 (non_max_suppression_obb) —
 TEST INFRASTRUCTURE.  torch CPU ops for the filtering, the pinned C++ oracle for the rotated NMS
 (mode 1 = reference CUDA rule `>`, mode 0 = reference CPU rule `>=`).  Pinned by
 tests/golden/postprocess_golden.npz (outputs of the reference function itself)."""

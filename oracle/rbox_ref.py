@@ -1,4 +1,4 @@
-"""numpy/torch-CPU restatement of /root/reference/utils/rboxs_utils.py:9-26,106-165 and
+"""numpy/torch-CPU restatement of utils/rboxs_utils.py:9-26,106-165 and
 utils/general.py:636-650 — TEST INFRASTRUCTURE.  Pinned by tests/golden/rbox_golden.npz."""
 import numpy as np
 
@@ -42,7 +42,7 @@ def scale_polys(img1_shape, polys, img0_shape):
 
 # ---------------------------------------------------------------------------------------------------------------
 # poly2rbox (utils/rboxs_utils.py:39-81).  Its arithmetic is cv2.minAreaRect — a third-party dependency that is not
-# under /root/reference: opencv-python >= 4.5.4 (requirements.txt:6, no lock file; 4.13.0 in the authoring container).
+# of the reference: opencv-python >= 4.5.4 (requirements.txt:6, no lock file).
 # Published algorithm (modules/imgproc/src/rotcalipers.cpp): convex hull, then the enclosing rectangle of minimum area
 # has a side collinear with a hull edge (rotating calipers); since 4.5.1 the returned angle lies in (0, 90] and `width`
 # is the side along that direction.  Restated here edge by edge in float64 and anchored on the reference's own call site

@@ -10,12 +10,12 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
 def ref_ext():
-    """The reference's own NMS kernels compiled from /root/reference into oracle/_ref (pinning)."""
+    """The reference's own NMS kernels compiled by oracle/build_ref.py into oracle/_ref (pinning)."""
     from oracle.build_ref import load_ref
     try:
         return load_ref()

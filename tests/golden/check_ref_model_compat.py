@@ -1,22 +1,19 @@
 """INTEGRATION.md B3, option 2 ("keep the reference Model object, replace _forward_once by InferenceEngine"): the engine
-identifies modules by class NAME and reads a fixed set of attributes (engine.py).  This script - authoring container only,
-it imports the REFERENCE package from /root/reference - builds the reference's Model and the mirror from the same yaml and
+identifies modules by class NAME and reads a fixed set of attributes (engine.py).  This script - needs the reference checkout,
+it imports the REFERENCE package (tests/golden/ref_import.py) - builds the reference's Model and the mirror from the same yaml and
 checks that the engine's view of the two is identical, attribute by attribute, and that the reference's state_dict loads
-into the mirror strictly (option 1).  Run by tests/test_ref_model_compat.py in a subprocess (the reference package puts
-top-level `models` / `utils` on sys.path and changes the working directory)."""
+into the mirror strictly (option 1).  It also stores what it compared - the reference's engine view, strides and parameter
+names / shapes - as tests/golden/ref_model_view.json, which tests/test_ref_model_compat.py checks the mirror against.
+Run as a script (the reference package puts top-level `models` / `utils` on sys.path and changes the working directory)."""
+import json
 import sys
 from pathlib import Path
 
 import torch
 
 HERE = Path(__file__).resolve().parent
-sys.path.insert(0, str(HERE))
-import ref_import  # noqa: E402
-
-ref_import.setup()
-sys.path.insert(0, str(HERE.parents[1]))
-from models.yolo import Model as RefModel  # noqa: E402  (the reference)
-from yolov5_obb_b200.yolo import Model as MirrorModel  # noqa: E402
+GOLDEN = HERE / "ref_model_view.json"
+SIZES = ("n", "s", "m")
 
 
 def conv_view(m):
@@ -57,8 +54,22 @@ def engine_view(model):
     return out
 
 
+def record(model):
+    """what is compared, in JSON form"""
+    return json.loads(json.dumps({"view": engine_view(model), "stride": [round(float(s), 6) for s in model.stride],
+                                  "params": [[n, list(p.shape)] for n, p in model.named_parameters()],
+                                  "state_dict": sorted(model.state_dict().keys())}))
+
+
 def main():
-    for size in ("n", "s", "m"):
+    sys.path.insert(0, str(HERE))
+    import ref_import
+    ref_import.setup()
+    sys.path.insert(0, str(HERE.parents[1]))
+    from models.yolo import Model as RefModel  # (the reference)
+    from yolov5_obb_b200.yolo import Model as MirrorModel
+    golden = {}
+    for size in SIZES:
         torch.manual_seed(0)
         ref = RefModel(f"models/yolov5{size}.yaml", ch=3, nc=15)
         torch.manual_seed(0)
@@ -72,7 +83,9 @@ def main():
         assert not missing.missing_keys and not missing.unexpected_keys
         for (na, pa), (nb, pb) in zip(ref.named_parameters(), mir.named_parameters()):
             assert na == nb and pa.shape == pb.shape, (na, nb)
+        golden[size] = record(ref)
         print(f"yolov5{size}: {len(a)} layers, {sum(p.numel() for p in ref.parameters())} parameters - identical engine view")
+    GOLDEN.write_text(json.dumps(golden, separators=(",", ":")) + "\n")
     print("COMPAT OK")
 
 

@@ -1,8 +1,8 @@
 """Generates the committed golden fixtures by running the REFERENCE's own code in the authoring
-container (where /root/reference exists).  Re-run: python tests/golden/make_golden.py
+container (where the reference checkout exists, oracle/build_ref.REF).  Re-run: python tests/golden/make_golden.py
 
   nms_golden.npz     keep lists of the reference CPU extension (nms_rotated_cpu.cpp, `>=`, host hull) built
-                     from /root/reference into oracle/_ref, on seeded inputs; each case is margin-checked
+                     from the reference checkout into oracle/_ref, on seeded inputs; each case is margin-checked
                      (no decisive IoU within 1e-4 of thr) so the `>`/`>=` and FMA differences cannot flip it
   iou_golden.npz     single_box_iou_rotated<float> host values (through a 2-box NMS probe is not possible,
                      so values come from the pinned C++ oracle, which the pin test ties to the reference
@@ -32,7 +32,7 @@ def margin_ok(d, s, thr, keep):
 
 
 def main():
-    assert build(), "needs /root/reference"
+    assert build(), "needs the reference checkout (oracle/build_ref.REF)"
     ref = load_ref()
     out = {}
     cases = [("dense300", 300, 200, 0.4, 2), ("dense1000", 1000, 300, 0.45, 3), ("cls15_2000", 2000, 1024, 0.4, 15),

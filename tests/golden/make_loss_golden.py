@@ -18,18 +18,18 @@ from models.yolo import Model  # noqa: E402
 from tests.lossgen import synth_preds, synth_targets  # noqa: E402
 
 # in-memory source shim: torch >= 1.12 refuses clamp_ with a float tensor bound (loss.py:267)
-src = Path("/root/reference/utils/loss.py").read_text()
+src = (ref_import.REF / "utils" / "loss.py").read_text()
 src = src.replace("gj.clamp_(0, feature_wh[1] - 1), gi.clamp_(0, feature_wh[0] - 1)",
                   "gj.clamp_(0, int(feature_wh[1]) - 1), gi.clamp_(0, int(feature_wh[0]) - 1)")
 assert "int(feature_wh[1])" in src
 mod = types.ModuleType("ref_loss")
 mod.__dict__["__name__"] = "utils.loss_shimmed"
-exec(compile(src, "/root/reference/utils/loss.py", "exec"), mod.__dict__)
+exec(compile(src, str(ref_import.REF / "utils" / "loss.py"), "exec"), mod.__dict__)
 
 
 def main():
     out = {}
-    hyp = yaml.safe_load(Path("/root/reference/data/hyps/obb/hyp.finetune_dota.yaml").read_text())
+    hyp = yaml.safe_load((ref_import.REF / "data" / "hyps" / "obb" / "hyp.finetune_dota.yaml").read_text())
     from tests.losscases import CASES as cases
     for name, c in cases.items():
         torch.manual_seed(0)

@@ -1,5 +1,5 @@
 """Golden vectors for poly2rbox from the REFERENCE's utils/rboxs_utils.py:39-81 (whose arithmetic is cv2.minAreaRect,
-opencv-python 4.13.0 in the authoring container; requirements.txt:6 only gives a lower bound >= 4.5.4).
+opencv-python 4.13.0 when they were made; requirements.txt:6 only gives a lower bound >= 4.5.4).
 python tests/golden/make_p2r_golden.py"""
 import sys
 from pathlib import Path

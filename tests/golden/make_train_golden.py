@@ -1,5 +1,5 @@
 """Golden vectors from the REFERENCE model in TRAIN mode (models/yolo.py Model: batch-statistic BatchNorm, raw Detect
-outputs, autograd backward as train.py:324-333 drives it) - run in the authoring container:
+outputs, autograd backward as train.py:324-333 drives it) - run where the reference checkout exists:
     python tests/golden/make_train_golden.py
 Writes train_golden.npz for yolov5n (nc=15, torch seed 0, tests/modelgen.seeded_state): the three training outputs on a
 seeded 2x3x64x96 batch; for every parameter gradient of a fixed linear functional of them its fp64 norm, its fp64 dot

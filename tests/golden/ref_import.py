@@ -1,4 +1,4 @@
-"""Import the REFERENCE python package from /root/reference (authoring container only) with the
+"""Import the REFERENCE python package from the reference checkout (oracle/build_ref.REF) with the
 environment shims SURVEY §8(c) lists: stub matplotlib/seaborn, cwd at the reference root (Arial.ttf),
 numpy.int alias, and the reference's nms_rotated_ext provided by oracle/_ref (its own CPU kernel).
 Used only by the make_*_golden.py scripts."""
@@ -8,12 +8,13 @@ import tempfile
 import types
 from pathlib import Path
 
-REF = Path("/root/reference")
 ROOT = Path(__file__).resolve().parents[2]
+sys.path.insert(0, str(ROOT))
+from oracle.build_ref import REF  # noqa: E402
 
 
 def setup():
-    assert REF.exists(), "the reference is only mounted in the authoring container"
+    assert REF.exists(), f"the reference checkout {REF} is missing"
     stubs = Path(tempfile.mkdtemp(prefix="refstubs_"))
     (stubs / "matplotlib").mkdir()
     (stubs / "matplotlib" / "__init__.py").write_text(

@@ -1,4 +1,4 @@
-"""GPU parity tests for the tcgen05 implicit-GEMM convolution, through the C ABI.
+"""GPU parity tests for the wgmma implicit-GEMM convolution, through the C ABI.
 
 Floating-point kernel: the reference is plain PyTorch fp32 (F.conv2d on the same bf16-rounded inputs
 and weights, then bias / SiLU / residual as models/common.py:37-49,94-104 and the Detect decode of
@@ -131,10 +131,10 @@ def test_conv_slices_residual_and_upsample():
 
 
 @pytest.mark.parametrize("cout,hw", [(32, 40), (64, 24), (256, 16)])
-def test_inplace_residual_reduce_add_equals_epilogue_add(cout, hw):
-    """The Bottleneck chain adds in place (out = res).  Default: the tile is ADDED into memory by the TMA store (bf16 add at L2, the
-    epilogue loads no residual); flag NO_RES_RED (16384): the epilogue loads the residual and adds in fp32.  Both must match the fp32
-    reference within the kernel's tolerance, and each other within one extra bf16 rounding of the sum."""
+def test_inplace_residual_add(cout, hw):
+    """The Bottleneck chain adds in place (out = res): the epilogue loads the residual from the output slice, adds it in fp32
+    and stores over it.  The result must match the fp32 reference within the kernel's tolerance, and the channels of the
+    wider buffer outside the slice must stay untouched."""
     from yolov5_obb_b200.conv import Conv, Slice, pack_weights
     B, H, W = 2, hw, hw + 8
     g = torch.Generator(device="cpu").manual_seed(11)
@@ -143,18 +143,11 @@ def test_inplace_residual_reduce_add_equals_epilogue_add(cout, hw):
     wp, bp = pack_weights(w, b)
     x = _mk(B, H, W, cout, 21)
     res0 = _mk(B, H, W, 2 * cout, 22)
-    outs = []
-    for flags in (0, 16384):
-        buf = res0.clone()                      # the chain lives in channels [0, cout) of a wider (concat) buffer
-        Conv(Slice.full(x), wp, bp, cout, 3, 1, 1, True, out=Slice(buf, 0, cout), res=Slice(buf, 0, cout), flags=flags).run()
-        torch.cuda.synchronize()
-        _check(buf[..., :cout], _ref_conv(x, w, b, 1, 1, True, res=res0[..., :cout]), f"in-place residual flags={flags}")
-        assert torch.equal(buf[..., cout:], res0[..., cout:]), "neighbouring channels untouched"
-        outs.append(buf[..., :cout].float())
-    # one extra rounding of the conv + SiLU term (= sum - residual) to bf16, then both sums round to bf16
-    d = (outs[0] - outs[1]).abs()
-    bound = 2.0 ** -8 * (outs[1] - res0[..., :cout].float()).abs() + 2.0 ** -7 * outs[1].abs() + 1e-3
-    assert bool((d <= bound).all()), "reduce-add differs from the fp32 add by more than one bf16 rounding"
+    buf = res0.clone()                      # the chain lives in channels [0, cout) of a wider (concat) buffer
+    Conv(Slice.full(x), wp, bp, cout, 3, 1, 1, True, out=Slice(buf, 0, cout), res=Slice(buf, 0, cout)).run()
+    torch.cuda.synchronize()
+    _check(buf[..., :cout], _ref_conv(x, w, b, 1, 1, True, res=res0[..., :cout]), "in-place residual")
+    assert torch.equal(buf[..., cout:], res0[..., cout:]), "neighbouring channels untouched"
 
 
 @pytest.mark.parametrize("decode", [True, False])

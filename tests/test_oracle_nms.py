@@ -1,5 +1,5 @@
-"""CPU tests: the oracle against the committed golden vectors and (where oracle/_ref is present)
-against the reference's own CPU extension compiled from /root/reference."""
+"""CPU tests: the oracle against the committed golden vectors and against the keep lists of the reference's own CPU
+extension (oracle/build_ref.py), stored in tests/golden/ref_kernels.npz (tests/refgold.py)."""
 from pathlib import Path
 
 import numpy as np
@@ -8,6 +8,7 @@ import torch
 
 import oracle
 from tests.boxgen import rboxes, degenerate_pairs
+from tests.refgold import reference
 
 ROOT = Path(__file__).resolve().parents[1]
 
@@ -36,9 +37,13 @@ def test_oracle_matches_golden_iou_values():
 
 @pytest.mark.parametrize("n,span,thr,seed", [(400, 250, 0.4, 0), (1500, 800, 0.3, 1), (900, 5000, 0.45, 2),
                                              (257, 100, 0.6, 3)])
-def test_oracle_pinned_to_reference_cpu_extension(ref_ext, n, span, thr, seed):
+def test_oracle_pinned_to_reference_cpu_extension(n, span, thr, seed):
     d, s, _ = rboxes(n, span, seed, n_classes=4)
-    ref = ref_ext.nms_rotated_cpu(torch.from_numpy(d), torch.from_numpy(s), thr).numpy()
+
+    def ref_cpu():
+        from oracle.build_ref import load_ref
+        return load_ref().nms_rotated_cpu(torch.from_numpy(d), torch.from_numpy(s), thr).numpy()
+    ref = reference(f"nms_cpu/{n}-{span}-{thr}-{seed}", ref_cpu)
     assert np.array_equal(oracle.nms_rotated(d, s, thr, mode=0), ref)
 
 

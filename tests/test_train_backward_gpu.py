@@ -1,4 +1,4 @@
-"""GPU parity of the training backward pass (BN/SiLU backward, tcgen05 dgrad + wgrad, pool / upsample / Detect
+"""GPU parity of the training backward pass (BN/SiLU backward, wgmma dgrad + wgrad, pool / upsample / Detect
 backward) against autograd over the fp32 oracle (oracle/model_ref), which is what the reference runs under
 train.py:333.
 

@@ -88,7 +88,7 @@ WG_CASES = [
 
 @pytest.mark.parametrize("B,Cin,Cout,H,W,k,s,xe,ze", WG_CASES)
 def test_wgrad_matches_autograd(B, Cin, Cout, H, W, k, s, xe, ze):
-    """tcgen05 wgrad straight from NHWC slices == autograd's conv2d weight gradient on the same bf16-rounded operands."""
+    """wgmma wgrad straight from NHWC slices == autograd's conv2d weight gradient on the same bf16-rounded operands."""
     from yolov5_obb_b200.train_ops import Wgrad
     p = k // 2
     Ho, Wo = (H + 2 * p - k) // s + 1, (W + 2 * p - k) // s + 1

@@ -1,4 +1,4 @@
-"""yolov5_obb_b200 — B200-native (sm_100a) engine behind yolov5_obb's hot-path entry points.
+"""yolov5_obb_b200 — H100-native (sm_90a) engine behind yolov5_obb's hot-path entry points.
 
 Only what the hot path needs lives here: csrc/ (CUDA kernels + the C ABI of include/y5obb.h) and the
 host-side mirrors of the reference operator interfaces (nms_rotated, general, loss, yolo).

@@ -14,7 +14,7 @@ _LIBPATH = _PKG / "liby5obb.so"
 _lib = None
 
 _ERR = {1: "Y5OBB_EINVAL (bad argument)", 2: "Y5OBB_EWORKSPACE (workspace too small)",
-        3: "Y5OBB_ECUDA (CUDA call failed)", 4: "Y5OBB_EARCH (device is not sm_100)"}
+        3: "Y5OBB_ECUDA (CUDA call failed)", 4: "Y5OBB_EARCH (device is not sm_90)"}
 
 # name -> (restype, argtypes); mirrors include/y5obb.h one to one (tests/test_abi.py checks the set)
 PROTOTYPES = {
@@ -40,9 +40,6 @@ PROTOTYPES = {
     "y5obb_conv_info": (c_int, [c_void_p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]
                         + [ctypes.POINTER(c_int)] * 4),
     "y5obb_conv_destroy": (None, [c_void_p]),
-    "y5obb_conv_debug_timestamps": (c_int, [c_void_p, c_void_p]),
-    "y5obb_wgrad_debug_occupancy": (c_int, [c_size_t] + [ctypes.POINTER(c_int)] * 2),
-    "y5obb_conv_debug_occupancy": (c_int, [c_int, c_int, c_size_t] + [ctypes.POINTER(c_int)] * 3),
     "y5obb_loss_workspace_bytes": (c_size_t, [c_void_p]),
     "y5obb_loss_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "y5obb_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

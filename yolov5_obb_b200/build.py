@@ -1,6 +1,6 @@
-"""Builds liby5obb.so (all CUDA kernels + the C ABI) for sm_100a with nvcc, in-tree.
+"""Builds liby5obb.so (all CUDA kernels + the C ABI) for sm_90a (H100) with nvcc, in-tree.
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU; the .so and the objects are build products (git-ignored).
 """
 import os
 import subprocess
@@ -14,7 +14,7 @@ OBJ = PKG.parent / "build" / "obj"
 LIB = PKG / "liby5obb.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -50,7 +50,7 @@ def build_lib(force: bool = False, verbose: bool = False) -> Path:
             list(ex.map(cc, jobs))
     objs = [OBJ / (s.stem + ".o") for s in srcs]
     if jobs or not LIB.exists():
-        cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", str(LIB), *map(str, objs)]
+        cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", str(LIB), *map(str, objs)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

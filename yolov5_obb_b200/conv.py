@@ -1,4 +1,4 @@
-"""Host-side handle for the tcgen05 implicit-GEMM convolution (csrc/conv_sm100.cu) behind the C ABI.
+"""Host-side handle for the wgmma implicit-GEMM convolution (csrc/conv_sm90.cu) behind the C ABI.
 
 A `Slice` names a channel range of an NHWC bf16 buffer; convs read and write slices, which is how
 Concat (models/common.py:267-274) disappears: producers store at a channel offset.

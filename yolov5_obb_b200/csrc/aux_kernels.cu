@@ -1,7 +1,7 @@
 // HBM-bound helpers around the conv stack (NHWC bf16):
 //   y5obb_stem_s2d     NCHW fp32 image -> 2x2 space-to-depth NHWC bf16 [B, H/2, W/2, 16] (12 real + 4 zero
 //                      channels), which turns the 6x6/s2/p2 stem conv (models/yolov5*.yaml layer 0,
-//                      models/common.py:37-49) into a 3x3/s1/p1 conv with K = 9 x 16 that the tcgen05
+//                      models/common.py:37-49) into a 3x3/s1/p1 conv with K = 9 x 16 that the wgmma
 //                      kernel runs with 32-byte swizzled tiles.
 //   y5obb_sppf_pool    the three chained 5x5/s1/p2 max-pools of SPPF (models/common.py:181-196) in one
 //                      pass: y1 = 5x5, y2 = 9x9, y3 = 13x13 windows of x (max-pool composition), written

@@ -1,9 +1,9 @@
 // Training-mode BatchNorm + SiLU around the tensor-core convolution (NHWC bf16), forward and backward.
-// Replaces the cuDNN/ATen batch_norm + SiLU kernels behind /root/reference/models/common.py:45-46
+// Replaces the cuDNN/ATen batch_norm + SiLU kernels behind models/common.py:45-46
 // (Conv.forward = act(bn(conv(x)))) in train mode (train.py:324-333), with BN eps = 1e-3 and momentum = 0.03
 // (utils/torch_utils.py:160-162).
 //
-// forward:   z = conv(x) (tensor-core kernel, raw bf16)                     [conv_sm100.cu]
+// forward:   z = conv(x) (tensor-core kernel, raw bf16)                     [conv_sm90.cu]
 //            k_bn_stats      per-channel sum / sum of squares of z (fp32 atomics, one pass over z)
 //            k_bn_finalize   mean, biased var -> scale = gamma / sqrt(var + eps), shift = beta - mean * scale;
 //                            running_mean / running_var update (unbiased var), as torch.nn.BatchNorm2d

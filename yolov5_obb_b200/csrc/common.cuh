@@ -1,4 +1,4 @@
-// Shared host/device helpers for liby5obb (sm_100a only).
+// Shared host/device helpers for liby5obb (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -44,8 +44,8 @@ inline int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }

@@ -1,6 +1,6 @@
 // ComputeLoss for the OBB head on the device: build_targets + CIoU box + obj/cls BCE + 180-bin CSL theta BCE,
-// forward and backward.  Replaces /root/reference/utils/loss.py:122-192 (__call__), :194-275 (build_targets)
-// and /root/reference/utils/metrics.py:201-236 (bbox_iou, CIoU), which run as ~60 small ATen kernels with
+// forward and backward.  Replaces utils/loss.py:122-192 (__call__), :194-275 (build_targets)
+// and utils/metrics.py:201-236 (bbox_iou, CIoU), which run as ~60 small ATen kernels with
 // three host syncs per level (boolean-mask indexing) and materialise a dense zero gradient through autograd.
 //
 //   k_match     one thread per (level, offset k, anchor a, target t) candidate: anchor-ratio test (:237-240)

@@ -1,7 +1,7 @@
-// Device-resident rotated NMS for sm_100a.
+// Device-resident rotated NMS for sm_90a.
 //
 // Replaces the reference's sort -> 64x64 IoU bit-matrix -> N^2/8-byte D2H -> serial host scan
-// (/root/reference/utils/nms_rotated/src/nms_rotated_cuda.cu:71-134) with five launches that never
+// (utils/nms_rotated/src/nms_rotated_cuda.cu:71-134) with five launches that never
 // leave the GPU:
 //   k_make_keys   64-bit key = (image << 32) | ~orderable(score); value = input index
 //   cub radix     one stable sort orders every image's boxes by descending score (ties: lower index)
@@ -9,7 +9,7 @@
 //   k_prep        per-box trig/area/circumradius once (the reference recomputes them per pair)
 //   k_tiles       persistent CTAs pull (row block, 8 col blocks) units of the UPPER triangle only;
 //                 phase 1 = exact far-pair reject into a shared-memory candidate list,
-//                 phase 2 = all lanes evaluate candidates with the bit-faithful IoU (rbox_iou.cuh),
+//                 phase 2 = all lanes evaluate candidates with the restated reference IoU (rbox_iou.cuh),
 //                 phase 3 = one 64-bit mask word per row
 //   k_reduce      one CTA per image runs the greedy scan over the bit-matrix in shared memory and
 //                 writes the compacted keep list in score order
@@ -228,7 +228,7 @@ k_tiles(const PreBox* __restrict__ pre, const NmsSeg* __restrict__ seg, int n_im
     for (int i = tid; i < TB * CHUNK; i += TILE_THREADS) s_mask[i] = 0ull;
     if (tid == 0) s_ncand = 0;
 
-    // phase 2 (all lanes busy): evaluate the buffered candidates with the bit-faithful IoU
+    // phase 2 (all lanes busy): evaluate the buffered candidates with the restated reference IoU
     auto drain = [&]() {
       __syncthreads();
       const int nc = s_ncand;
@@ -671,7 +671,7 @@ int nms_impl(const float* dets, const float* scores, const int32_t* image_ids, i
 
 
 // ---------------------------------------------------------------------------------------------
-// non_max_suppression_obb on the device (/root/reference/utils/general.py:772-862)
+// non_max_suppression_obb on the device (utils/general.py:772-862)
 //   k_pp_count   one warp per anchor row: obj > conf (:781,:804), conf = cls * obj (:820), per-class
 //                candidates when multi_label (:826-828) or the best class (:830-832), class filter (:835)
 //   cub scan     deterministic candidate offsets in (image, anchor, class) order == the reference's order
@@ -1166,7 +1166,7 @@ extern "C" {
 
 int y5obb_abi_version(void) { return 1; }
 int y5obb_last_cuda_error(void) { return g_last_cuda_error; }
-const char* y5obb_build_info(void) { return "liby5obb sm_100a " __DATE__ " " __TIME__; }
+const char* y5obb_build_info(void) { return "liby5obb sm_90a " __DATE__ " " __TIME__; }
 
 size_t y5obb_nms_workspace_bytes(int64_t n_total, int64_t n_images, int64_t max_per_image) {
   if (n_total <= 0) return 256;

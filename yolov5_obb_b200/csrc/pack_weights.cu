@@ -1,6 +1,6 @@
 // Re-packing of the fp32 master weights into the bf16 operand layouts of the tensor-core kernels, all layers in ONE
 // launch.  Training updates the parameters every step (train.py:336), so the packed copies the TMA descriptors point at
-// must be refreshed every step: forward layout [tap][cout_pad][cin_pad] (K-major B operand of conv_sm100.cu) and the
+// must be refreshed every step: forward layout [tap][cout_pad][cin_pad] (K-major B operand of conv_sm90.cu) and the
 // data-gradient layout (the same kernel run with the weights transposed and the taps flipped).
 // One thread per packed element; a table of entries (device resident, built once per plan) tells it where the element
 // comes from.  HBM-bound: 4 B read + 2 B written per packed element.

@@ -1,13 +1,13 @@
 // Float polygon NMS and rotated-box overlaps of the DOTA devkit / the nms_rotated extension (SURVEY section 8 rows A14, B4):
-//   /root/reference/DOTA_devkit/poly_nms_gpu/poly_nms_kernel.cu:214-264 (K3 kernel), :277-329 (_poly_nms host entry)
-//   /root/reference/DOTA_devkit/poly_nms_gpu/poly_overlaps_kernel.cu:283-353 (RotBox2Poly, K4 kernel), :368-427 (_overlaps)
-//   /root/reference/utils/nms_rotated/src/poly_nms_cuda.cu:144-261 (K2 = the same kernel behind nms_rotated_ext.nms_poly,
+//   DOTA_devkit/poly_nms_gpu/poly_nms_kernel.cu:214-264 (K3 kernel), :277-329 (_poly_nms host entry)
+//   DOTA_devkit/poly_nms_gpu/poly_overlaps_kernel.cu:283-353 (RotBox2Poly, K4 kernel), :368-427 (_overlaps)
+//   utils/nms_rotated/src/poly_nms_cuda.cu:144-261 (K2 = the same kernel behind nms_rotated_ext.nms_poly,
 //   unbuildable on torch >= 1.11 because it needs THC)
 // All three share one float polygon IoU (triangle fans about the origin, half-plane cuts, eps = 1e-8 sign tests evaluated in
 // double).  Parity contract: every floating-point expression below has the operand order and float/double mix of the
 // reference expression it restates, and this file is compiled with nvcc's default -fmad=true like the reference, so the
 // fused/unfused rounding pattern is the same; tests/test_poly_f32_gpu.py compares IoU matrices bit for bit and keep lists
-// against the reference kernels compiled from /root/reference for sm_100a (oracle/_ref/libref_polygpu_*.so).
+// against the reference kernels compiled by oracle/build_ref.py for sm_90a (oracle/_ref/libref_polygpu_*.so).
 //
 // What is NOT the reference's design: only the upper triangle of the 64x64 block grid is evaluated (the reference computes
 // the full grid and ignores the lower half), the greedy scan runs on the device (the reference copies the N^2/8-byte matrix

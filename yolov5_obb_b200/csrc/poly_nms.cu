@@ -1,8 +1,8 @@
 // Tile-merge polygon NMS of the DOTA devkit on the device (SURVEY section 8f rank 4, row A14's CPU form):
-//   /root/reference/DOTA_devkit/ResultMerge_multi_process.py:62-123  py_cpu_nms_poly_fast
-//   /root/reference/DOTA_devkit/polyiou.cpp:9-128                    iou_poly (double, eps = 1e-8 sign tests)
+//   DOTA_devkit/ResultMerge_multi_process.py:62-123  py_cpu_nms_poly_fast
+//   DOTA_devkit/polyiou.cpp:9-128                    iou_poly (double, eps = 1e-8 sign tests)
 // Written against the bit-equal CPU restatement (oracle/poly_ref.py, pinned to the reference's polyiou.cpp compiled in
-// place); on the B200 tests/test_poly_gpu.py finds the IoUs bit-equal and the keep lists equal to the reference's.
+// place); tests/test_poly_gpu.py checks the IoUs bit-equal and the keep lists equal to the reference's.
 //
 // Pipeline: CUB radix sort by descending score (stable, ties -> lower index, as numpy's argsort()[::-1] is NOT: the
 // reference's tie order is the reverse index order; callers with tied scores get the documented lower-index-first rule) ->

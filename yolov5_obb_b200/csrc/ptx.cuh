@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the conv kernels use: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (TMEM alloc / mma / commit / ld) and the proxy fences between them.
+// Thin inline-PTX wrappers for the sm_90a features the conv kernels use: mbarrier, TMA (cp.async.bulk.tensor), the wgmma
+// shared-memory descriptors (wgmma.cuh has the MMAs) and the proxy fences between them.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -138,82 +138,30 @@ __device__ __forceinline__ void tma_store_wait_read() {
 }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- tcgen05 / TMEM -------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate, single CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives columns [c, c+32) of lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA descriptors -----------------------------------------------------------------------
-// K-major operand tile in shared memory, rows of `row_bytes` (= 32, 64 or 128, equal to the TMA
-// swizzle span), 8-row groups `8 * row_bytes` apart.  Bit layout: cute/arch/mma_sm100_desc.hpp
-// (SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-// layout_type [61,64) (2 = 128B, 4 = 64B, 6 = 32B swizzle).
+// ---- wgmma shared-memory descriptors ----------------------------------------------------------
+// Bit layout (PTX ISA, "Matrix Descriptor Format" of wgmma): start address >> 4 [0,14), leading byte offset >> 4 [16,30),
+// stride byte offset >> 4 [32,46), base offset [49,52) (0: every tile starts on a swizzle-pattern boundary), swizzle mode
+// [62,64) (1 = 128B, 2 = 64B, 3 = 32B).
+// K-major operand tile: rows of `row_bytes` (= 32, 64 or 128, equal to the TMA swizzle span), 8-row groups `8 * row_bytes`
+// apart (SBO); the leading offset is unused for swizzled K-major tiles.
 __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, uint32_t row_bytes) {
-  const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
+  const uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;                              // LBO (ignored for swizzled K-major)
-  d |= (uint64_t)((8u * row_bytes) >> 4) << 32;        // SBO
-  d |= (uint64_t)1 << 46;                              // descriptor version (Blackwell)
-  d |= layout << 61;
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((8u * row_bytes) >> 4) << 32;
+  d |= layout << 62;
   return d;
 }
-
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32, both operands K-major
-// (InstrDescriptor in mma_sm100_desc.hpp): c_format [4,6)=1, a_format [7,10)=1, b_format [10,13)=1,
-// n>>3 [17,23), m>>4 [24,29).
-__host__ __device__ inline uint32_t make_idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+// MN-major, 128B-swizzled operand: 64-element chunks of [K rows][128 B]; chunks `chunk` bytes apart along M / N (LBO),
+// 8-row K groups 1024 B apart (SBO).
+__device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32_t chunk) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)(chunk >> 4) << 16;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
 
 }  // namespace ptx

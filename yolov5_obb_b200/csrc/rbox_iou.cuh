@@ -1,12 +1,13 @@
-// Rotated-box IoU for sm_100a — device restatement of the reference's *device* code path
-//   /root/reference/utils/nms_rotated/src/box_iou_rotated_utils.h:57-360 (the __CUDACC__ branch:
+// Rotated-box IoU for sm_90a — device restatement of the reference's *device* code path
+//   utils/nms_rotated/src/box_iou_rotated_utils.h:57-360 (the __CUDACC__ branch:
 //   exchange-sort hull ordering, :195-218), called per pair by nms_rotated_cuda.cu:57-62.
 //
 // Parity contract: every floating-point expression below has the same operand order and the same
 // float/double mix as the reference expression it restates (cited per block), and this file is
-// compiled with nvcc's default -fmad=true like the reference extension, so the fused/unfused
-// rounding pattern chosen by nvcc/ptxas is the same.  tests/test_nms_gpu.py checks IoU values bit
-// for bit against the reference device function compiled from /root/reference (oracle/_ref).
+// compiled with nvcc's default -fmad=true like the reference extension.  Which products ptxas fuses
+// into FMAs still depends on the surrounding program: on sm_90a 17.9 % of the IoUs of
+// tests/test_nms_gpu.py's 400 000 near pairs differ from the reference device function, by at most
+// 4 ulp; degenerate pairs and every tested keep list of the reference's CUDA kernel are equal.
 //
 // What is NOT the reference's design: trig and area are computed once per box (PreBox), not once per
 // pair; the caller rejects far-apart pairs before calling this (exact: such pairs have IoU == 0).

@@ -1,8 +1,8 @@
 // Post-NMS geometry and CSL targets (HBM-bound elementwise kernels; one thread per box):
-//   y5obb_rbox2poly_f32      /root/reference/utils/rboxs_utils.py:106-126  (torch branch of rbox2poly)
-//   y5obb_poly2hbb_f32       /root/reference/utils/rboxs_utils.py:147-165  (torch branch of poly2hbb)
-//   y5obb_scale_polys_f32    /root/reference/utils/general.py:636-650      (scale_polys, in place)
-//   y5obb_gaussian_label     /root/reference/utils/rboxs_utils.py:9-26     (gaussian_label_cpu: 180-bin CSL row)
+//   y5obb_rbox2poly_f32      utils/rboxs_utils.py:106-126  (torch branch of rbox2poly)
+//   y5obb_poly2hbb_f32       utils/rboxs_utils.py:147-165  (torch branch of poly2hbb)
+//   y5obb_scale_polys_f32    utils/general.py:636-650      (scale_polys, in place)
+//   y5obb_gaussian_label     utils/rboxs_utils.py:9-26     (gaussian_label_cpu: 180-bin CSL row)
 // Each arithmetic step is a separately rounded fp32 op (no FMA contraction), like the chain of ATen
 // elementwise kernels it replaces; the CSL row is evaluated in fp64 like the numpy original.
 #include <algorithm>

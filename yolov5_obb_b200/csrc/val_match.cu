@@ -1,7 +1,7 @@
 // Post-NMS geometry + validation matching of one batch in ONE launch (SURVEY section 8f rank 3):
-//   /root/reference/val.py:226-250 per image:  rbox2poly -> scale_polys -> poly2hbb -> xywh2xyxy for the detections,
+//   val.py:226-250 per image:  rbox2poly -> scale_polys -> poly2hbb -> xywh2xyxy for the detections,
 //       rbox2poly -> poly2hbb -> xywh2xyxy -> scale_coords (+ clip) for the labels, then
-//   /root/reference/val.py:69-92 process_batch:  HBB box_iou (utils/metrics.py:246-268), class match, IoU >= iouv[0]; every
+//   val.py:69-92 process_batch:  HBB box_iou (utils/metrics.py:246-268), class match, IoU >= iouv[0]; every
 //       detection keeps its highest-IoU label, every label keeps its lowest-index (= most confident) detection among those;
 //       correct[d, :] = iou >= iouv for the surviving pairs.
 // The reference runs ~40 small ATen kernels, two host round trips (numpy argsort / unique) and a Python loop per image.

@@ -1,4 +1,4 @@
-"""Inference plan: turns a yolo.Model into a fixed sequence of sm_100a kernel launches.
+"""Inference plan: turns a yolo.Model into a fixed sequence of sm_90a kernel launches.
 
 Layout decisions (all NHWC bf16):
   * every tensor is a channel slice of some buffer; a producer whose output feeds a Concat
@@ -54,7 +54,7 @@ class InferenceEngine:
     def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, conv_flags: int = 0, compact_detect: bool = False):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("InferenceEngine needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("InferenceEngine needs a CUDA device (sm_90a); there is no CPU path")
         det = model.model[-1]
         smax = int(max(model.stride))
         if H % smax or W % smax:

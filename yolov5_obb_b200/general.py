@@ -1,4 +1,4 @@
-"""Host-side mirror of /root/reference/utils/general.py:772-862 (non_max_suppression_obb) — same signature
+"""Host-side mirror of utils/general.py:772-862 (non_max_suppression_obb) — same signature
 and return value; the per-image Python loop, its >= 6 host syncs per image and the N^2/8-byte mask copy are
 replaced by one device pipeline (csrc/nms.cu: k_pp_* + batched rotated NMS) and ONE small D2H read of the
 per-image counts at the end."""

@@ -1,4 +1,4 @@
-"""Host-side mirror of /root/reference/utils/loss.py:90-192 ComputeLoss — same constructor and call
+"""Host-side mirror of utils/loss.py:90-192 ComputeLoss — same constructor and call
 signature, autograd-compatible (`scaler.scale(loss).backward()`, train.py:333), backed by csrc/loss.cu.
 
     compute_loss = ComputeLoss(model)            # reads model.hyp and the Detect module

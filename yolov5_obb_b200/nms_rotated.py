@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's rotated-NMS operator interface.
 
-Mirrors /root/reference/utils/nms_rotated/nms_rotated_wrapper.py:6-46 (obb_nms) and the pybind module
-/root/reference/utils/nms_rotated/src/nms_rotated_ext.cpp:25-59 (nms_rotated_ext.nms_rotated), same
+Mirrors utils/nms_rotated/nms_rotated_wrapper.py:6-46 (obb_nms) and the pybind module
+utils/nms_rotated/src/nms_rotated_ext.cpp:25-59 (nms_rotated_ext.nms_rotated), same
 names, argument meaning and error behaviour (RuntimeError on a failing op), but backed by the
 device-resident kernels in csrc/nms.cu through the C ABI (include/y5obb.h).
 """

@@ -1,11 +1,10 @@
-"""End-to-end detection pipeline from HOST images: the loop of /root/reference/detect.py:104-122 and
+"""End-to-end detection pipeline from HOST images: the loop of detect.py:104-122 and
 val.py:183-207 (pre-process, inference, NMS), software-pipelined:
 
 * `slots` batches are in flight at once, each on its own CUDA stream with its own plan (activation / record buffers, captured
   forward graph) and its own post-process graph.  The conv kernels are persistent one-CTA-per-SM launches whose ramps and tails
   leave SMs idle, and the NMS stage is a chain of small latency-bound kernels: a second batch on another stream fills both
-  (measured on B200, yolov5s b16 1024^2: 1.95 ms per step with one batch in flight, 1.71 with two, 1.69 with three -
-  tools/time_streams.py).  Results are bit-identical to the blocking calls: the same kernels run on the same data, only
+  (tools/time_streams.py compares slot counts).  Results are bit-identical to the blocking calls: the same kernels run on the same data, only
   their interleaving changes.
 * the host->device copy of batch i+1 runs on a copy stream while batch i computes (max(2, slots) device input buffers,
   event-ordered), and the device->host copy of batch i's detections is asynchronous, so the host turns batch i-slots into

@@ -1,4 +1,4 @@
-"""Host-side mirror of /root/reference/utils/rboxs_utils.py (tensor branches) and general.scale_polys, backed
+"""Host-side mirror of utils/rboxs_utils.py (tensor branches) and general.scale_polys, backed
 by csrc/rbox_utils.cu: rbox2poly (:106-126), poly2hbb (:147-165), gaussian_label (:9-26, on the device so
 that only [nt,7] targets need to cross PCIe — SURVEY §8f rank 2), scale_polys (utils/general.py:636-650)."""
 import torch

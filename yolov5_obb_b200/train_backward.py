@@ -1,6 +1,6 @@
 """Backward pass of the training plan (train_engine.TrainEngine): what autograd + cuDNN do under
-`scaler.scale(loss).backward()` (/root/reference/train.py:333) for the Conv/C3/SPPF/Concat/Upsample/Detect graph,
-as a fixed sequence of sm_100a kernel launches.
+`scaler.scale(loss).backward()` (train.py:333) for the Conv/C3/SPPF/Concat/Upsample/Detect graph,
+as a fixed sequence of sm_90a kernel launches.
 
 Per Conv module (y = [res +] silu(bn(conv(x))), reverse order):
    gy (+ 2x-up-sampled copy's gradient folded in)  --y5obb_bn_silu_bwd-->  dz, dgamma, dbeta, residual pass-through

@@ -1,5 +1,5 @@
 """Training-mode plan: Conv = tensor-core conv (raw) -> batch statistics -> normalise + SiLU, every intermediate
-kept for the backward pass.  Mirrors /root/reference/models/yolo.py:163-181 (_forward_once) in train mode
+kept for the backward pass.  Mirrors models/yolo.py:163-181 (_forward_once) in train mode
 (train.py:324-326): BatchNorm uses batch statistics (eps 1e-3) and updates its running statistics with momentum
 0.03 (utils/torch_utils.py:160-162); Detect returns the three raw [B, 3, H, W, no] tensors (yolo.py:62-65,81).
 
@@ -36,7 +36,7 @@ class TrainEngine:
     def __init__(self, model, B: int, H: int, W: int, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("TrainEngine needs a CUDA device (sm_100a); there is no CPU path")
+            raise RuntimeError("TrainEngine needs a CUDA device (sm_90a); there is no CPU path")
         det = model.model[-1]
         smax = int(max(model.stride))
         if H % smax or W % smax:

@@ -1,4 +1,4 @@
-"""One optimisation step of /root/reference/train.py:296-342 (the loop body), driven through the same entry points:
+"""One optimisation step of train.py:296-342 (the loop body), driven through the same entry points:
 
     pred = model(imgs)                       # models/yolo.py Model.forward   -> train_engine / train_backward kernels
     loss, items = compute_loss(pred, tgts)   # utils/loss.py ComputeLoss      -> csrc/loss.cu

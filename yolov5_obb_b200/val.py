@@ -1,4 +1,4 @@
-"""Host-side mirror of the per-image metric block of the reference's validation loop (/root/reference/val.py:209-250 and
+"""Host-side mirror of the per-image metric block of the reference's validation loop (val.py:209-250 and
 process_batch :69-92), executed for a whole batch by ONE kernel (csrc/val_match.cu, SURVEY section 8f rank 3)."""
 import torch
 

@@ -1,7 +1,7 @@
-"""Host-side mirror of the reference model interface, executed by the sm_100a engine.
+"""Host-side mirror of the reference model interface, executed by the sm_90a engine.
 
-Mirrors /root/reference/models/yolo.py (Model :95-268, Detect :33-92, parse_model :271-323) and the
-building blocks of /root/reference/models/common.py (Conv :37-49, Bottleneck :94-104, C3 :126-138,
+Mirrors models/yolo.py (Model :95-268, Detect :33-92, parse_model :271-323) and the
+building blocks of models/common.py (Conv :37-49, Bottleneck :94-104, C3 :126-138,
 SPPF :181-196, Concat :267-274): same constructor arguments, same module/parameter names (so a
 reference state_dict loads unchanged), same forward() return values.  The modules here only HOLD
 parameters; all arithmetic runs in csrc/ through the C ABI (engine.py).  There is no PyTorch compute
@@ -52,7 +52,7 @@ def autopad(k, p=None):
 class _NoTorchPath(nn.Module):
     def forward(self, *a, **k):  # pragma: no cover
         raise RuntimeError(f"{type(self).__name__} holds parameters only; run the model through "
-                           "yolov5_obb_b200.yolo.Model.forward (sm_100a engine) — there is no PyTorch fallback")
+                           "yolov5_obb_b200.yolo.Model.forward (sm_90a engine) — there is no PyTorch fallback")
 
 
 class Conv(_NoTorchPath):
