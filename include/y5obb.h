@@ -349,7 +349,37 @@ int y5obb_poly_nms_f64(const double* dets9, int64_t n, double thresh, int64_t* k
                        size_t workspace_bytes, void* stream);
 int y5obb_poly_iou_pairs_f64(const double* p8, const double* q8, double* iou_out, int64_t n, void* stream);
 
-/* ---- post-NMS geometry + validation matching (SURVEY 8f rank 3) ------------------------------------------------------
+/* ---- whole-scene inference: tile input and tile-merge (DOTA scenes larger than one tile) --------------------------------
+ * The reference's route (README.md:24-26): DOTA_devkit/ImgSplit_multi_process.py:226-273 cuts the scene into subsize^2 tiles
+ * (zero padding beyond the scene), val.py --save-json detects each one letterboxed to size^2 (114 border, utils/augmentations.py:
+ * 92-128; pad=0.5 rect batching), tools/TestJson2VocClassTxt.py and DOTA_devkit/ResultMerge_multi_process.py:62-236 shift the
+ * polygons into the scene and run py_cpu_nms_poly_fast per (scene, class).
+ *
+ * y5obb_scene_tiles_s2d_u8: scene_hwc [H, W, 3] uint8 BGR (as cv2.imread returns it; 64-bit addressing), origins2 [n_tiles, 2]
+ * int32 (left, up) -> the stem input of the n_tiles tiles in y5obb_stem_s2d_u8's layout [n_tiles, size/2, size/2 + 2*pad_cols, 16]:
+ * tile pixel (y, x) of the size^2 letterboxed tile is 114 outside [border, border + subsize)^2, else scene pixel
+ * (up + y - border, left + x - border) in RGB order, or 0 beyond the scene.  The pad_cols columns are not written. */
+int y5obb_scene_tiles_s2d_u8(const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles, int subsize,
+                             int size, int border, void* out_nhwc16, int pad_cols, void* stream);
+/* y5obb_scene_merge_f64: rows7 [n_tiles, max_det, 7] + counts [n_tiles] = the packed output of y5obb_nms_obb_f32 for the tiles
+ * (cx, cy, l, s, theta, conf, cls; counts[t] valid rows), origins2 as above -> out10 [K, 10] fp64 rows (class, score, x1 y1 ...
+ * x4 y4), per class (ascending) in keep order, *n_out = K (out10 holds n_tiles * max_det rows).  Per row, as the reference's
+ * chain computes it: rbox2poly (fp32), scale_polys (x - pad) / gain (fp32), Python round(x, 1) and round(conf, 5) of the fp32
+ * values, x + left / y + up in fp64; then per class py_cpu_nms_poly_fast at `thresh` over the candidates sorted by descending
+ * rounded score (ties: lower tile * max_det + row first).  Rows of a class outside [0, nc) are ignored.
+ * SYNCHRONOUS once: the per-class candidate counts are copied to class_cands_host [nc] (host memory) and the stream is
+ * synchronised, because they size the dense suppression masks that follow in the workspace.  Returns Y5OBB_EINVAL when a class
+ * has more than Y5OBB_SCENE_MAX_CLASS_CANDIDATES candidates (its dense mask would exceed 512 MiB), and Y5OBB_EWORKSPACE when
+ * y5obb_scene_merge_workspace_bytes(n_tiles, max_det, nc, class_cands_host) exceeds workspace_bytes (class_cands_host is
+ * filled in both cases; call again with a larger workspace).  With class_cands_host = NULL the query returns the part of the
+ * workspace needed before the counts are known. */
+#define Y5OBB_SCENE_MAX_CLASS_CANDIDATES 65536
+size_t y5obb_scene_merge_workspace_bytes(int64_t n_tiles, int max_det, int nc, const int64_t* class_cands_host);
+int y5obb_scene_merge_f64(const float* rows7, const int64_t* counts, const int32_t* origins2, int64_t n_tiles, int max_det,
+                          int nc, float pad, float gain, double thresh, double* out10, int64_t* n_out, int64_t* class_cands_host,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- post-NMS geometry + validation matching (SURVEY 8f rank 3)------------------------------------------------------
  * One launch per batch for val.py:226-250 + process_batch (val.py:69-92): detections pred7 [batch, max_det, 7] (the packed
  * output of y5obb_nms_obb_f32, counts[b] valid rows) -> native-space polygons polyn8 [batch, max_det, 8] (rbox2poly +
  * scale_polys) and boxes hbbn4 [batch, max_det, 4] (poly2hbb + xywh2xyxy) (either may be NULL), and correct

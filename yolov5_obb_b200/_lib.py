@@ -88,7 +88,14 @@ PROTOTYPES = {
     "y5obb_stem_s2d": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_stem_s2d_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_sppf_pool": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
+    "y5obb_scene_tiles_s2d_u8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                         c_void_p]),
+    "y5obb_scene_merge_workspace_bytes": (c_size_t, [c_int64, c_int, c_int, c_void_p]),
+    "y5obb_scene_merge_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_float, c_float, ctypes.c_double,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
+
+SCENE_MAX_CLASS_CANDIDATES = 65536  # Y5OBB_SCENE_MAX_CLASS_CANDIDATES
 
 NMS_STRICT_GT = 1
 NMS_DROP_SMALL = 2

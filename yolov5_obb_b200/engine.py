@@ -275,19 +275,28 @@ class InferenceEngine:
                 x = x.contiguous().float()
                 _lib.check(L.y5obb_stem_s2d(x.data_ptr(), self.x_s2d.data_ptr(), self.B, self.H, self.W, 1, st),
                            "y5obb_stem_s2d")
-            # the layer sequence is fixed (same buffers every call): from the third call on it is replayed as one CUDA
-            # graph - the layout pass above stays outside because it reads the caller's tensor (Y5OBB_NO_GRAPH=1 disables)
-            self._calls += 1
-            if self._use_graph and self._calls > 2:
-                if self._graph is None:
-                    torch.cuda.synchronize(self.device)
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        self._run_ops(_lib.stream_ptr(self.device))
-                    self._graph = g
-                self._graph.replay()
-            else:
-                self._run_ops(st)
+            return self._run_layers()
+
+    def forward_s2d(self) -> torch.Tensor:
+        """Runs the plan on an `x_s2d` the caller has already filled (y5obb_scene_tiles_s2d_u8 writes the stem input of
+        scene tiles there) -> pred (or the compact records), engine-owned as in forward()."""
+        with torch.cuda.device(self.device):
+            return self._run_layers()
+
+    def _run_layers(self) -> torch.Tensor:
+        # the layer sequence is fixed (same buffers every call): from the third call on it is replayed as one CUDA
+        # graph - the layout pass stays outside because it reads the caller's tensor (Y5OBB_NO_GRAPH=1 disables)
+        self._calls += 1
+        if self._use_graph and self._calls > 2:
+            if self._graph is None:
+                torch.cuda.synchronize(self.device)
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                    self._run_ops(_lib.stream_ptr(self.device))
+                self._graph = g
+            self._graph.replay()
+        else:
+            self._run_ops(_lib.stream_ptr(self.device))
         return self.pred
 
     def _run_ops(self, st):

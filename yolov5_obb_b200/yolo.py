@@ -327,17 +327,24 @@ class Model(nn.Module):
         tensor (bit-identical detections: same sigmoid / decode arithmetic, same first-maximum theta rule).
         `slot` selects one of several independent plans of the same shape (own activation and record buffers, own captured
         graph): batches in flight on DIFFERENT streams must use different slots (pipeline.DetectPipeline does)."""
+        from .general import DetectRecords
+        eng = self.records_plan(tuple(x.shape), x.device, slot)
+        return DetectRecords(eng.forward(x), eng.nc)
+
+    def records_plan(self, shape, device, slot: int = 0):
+        """The InferenceEngine behind detect_records for inputs of `shape` [B, 3, H, W] on `device`, re-planned when the weights
+        changed since it was built.  Callers that write the plan's `x_s2d` themselves run it with forward_s2d() (scene.py)."""
         if self.training:
             raise RuntimeError("detect_records is an inference entry point (model.eval())")
         from .engine import InferenceEngine
-        from .general import DetectRecords
-        key = ("records", tuple(x.shape), x.device.index) + ((int(slot),) if slot else ())
+        device = torch.device(device)
+        key = ("records", tuple(shape), device.index) + ((int(slot),) if slot else ())
         eng = self._engines.get(key)
         sig = self._weights_signature()
         if eng is None or eng._weights_sig != sig:
-            eng = self._engines[key] = InferenceEngine(self, x.shape[0], x.shape[2], x.shape[3], x.device, compact_detect=True)
+            eng = self._engines[key] = InferenceEngine(self, shape[0], shape[2], shape[3], device, compact_detect=True)
             eng._weights_sig = sig
-        return DetectRecords(eng.forward(x), eng.nc)
+        return eng
 
     def _weights_signature(self):
         tr = getattr(self, "_sig_tensors", None)
