@@ -379,6 +379,29 @@ int y5obb_scene_merge_f64(const float* rows7, const int64_t* counts, const int32
                           int nc, float pad, float gain, double thresh, double* out10, int64_t* n_out, int64_t* class_cands_host,
                           void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- DOTA Task1 evaluation (OBB mAP of the reference's README) ---------------------------------------------------------
+ * y5obb_dota_eval_f64: DOTA_devkit/dota_evaluation_task1.py:88-249 voc_eval + :54-85 voc_ap for every class at once.
+ * det10 [n_det, 10] fp64 = (class, score, x1 y1 ... x4 y4) with det_img [n_det] the image index (the layout of
+ * SceneDetections.rows); gt10 [n_gt, 10] fp64 = (class, difficult, x1 y1 ... x4 y4) with gt_img [n_gt], difficult non-zero =
+ * difficult.  Per class: detections in descending score (ties: lower input index first), each compared with the GTs of its
+ * (image, class) in input order through the axis-aligned pre-filter (+1 pixel convention on the intersection and the
+ * union) and iou_poly(GT, det); TP / FP / ignored as voc_eval's R['det'] loop decides them; rec = tp / npos,
+ * prec = tp / max(tp + fp, DBL_EPSILON); ap by the VOC07 11-point metric (use_07_metric != 0) or the continuous one, with
+ * numpy's pairwise summation.  Outputs (device): class_off [nc + 1] (class c's curve is rec / prec [class_off[c],
+ * class_off[c + 1])), rec / prec [n_det], ap [nc], npos [nc] (non-difficult GTs), status [1]: 0, or Y5OBB_EINVAL when a row's
+ * class is not an integer in [0, nc) or its image is outside [0, n_images) (such rows are left out; the outputs are then
+ * not meaningful).  Asynchronous: no host read, no synchronisation.  Returns Y5OBB_EINVAL for negative sizes, nc <= 0 or
+ * null pointers, Y5OBB_EWORKSPACE when ws_bytes < y5obb_dota_eval_workspace_bytes(n_det, n_gt, n_images, nc). */
+size_t y5obb_dota_eval_workspace_bytes(int64_t n_det, int64_t n_gt, int n_images, int nc);
+int y5obb_dota_eval_f64(const int32_t* det_img, const double* det10, int64_t n_det, const int32_t* gt_img, const double* gt10,
+                        int64_t n_gt, int n_images, int nc, double ovthresh, int use_07_metric, int64_t* class_off,
+                        double* rec, double* prec, double* ap, int64_t* npos, int32_t* status, void* ws, size_t ws_bytes,
+                        void* stream);
+/* y5obb_task1_round_f64: rows10 [n, 10] (class, score, 8 coordinates) -> out10 with Python's round(score, 2) and
+ * round(x, 1), the values the Task1 text of ResultMerge_multi_process.py mergesingle (:221-236) parses back to
+ * (dota_evaluation_task1.py:88-249 reads that text). */
+int y5obb_task1_round_f64(const double* rows10, int64_t n, double* out10, void* stream);
+
 /* ---- post-NMS geometry + validation matching (SURVEY 8f rank 3)------------------------------------------------------
  * One launch per batch for val.py:226-250 + process_batch (val.py:69-92): detections pred7 [batch, max_det, 7] (the packed
  * output of y5obb_nms_obb_f32, counts[b] valid rows) -> native-space polygons polyn8 [batch, max_det, 8] (rbox2poly +

@@ -93,6 +93,11 @@ PROTOTYPES = {
     "y5obb_scene_merge_workspace_bytes": (c_size_t, [c_int64, c_int, c_int, c_void_p]),
     "y5obb_scene_merge_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_float, c_float, ctypes.c_double,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "y5obb_dota_eval_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int, c_int]),
+    "y5obb_dota_eval_f64": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, ctypes.c_double,
+                                    c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                    c_void_p]),
+    "y5obb_task1_round_f64": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
 }
 
 SCENE_MAX_CLASS_CANDIDATES = 65536  # Y5OBB_SCENE_MAX_CLASS_CANDIDATES

@@ -1,6 +1,8 @@
 // Device geometry shared by several kernels:
 //   rbox2poly_f32      utils/rboxs_utils.py:106-126 in separately rounded fp32 ops (rbox_utils.cu, scene.cu)
-//   iou_poly_dev       DOTA_devkit/polyiou.cpp:9-128 iou_poly in fp64 without FMA contraction (poly_nms.cu, scene.cu)
+//   py_round           Python's round(x, n) on doubles, exactly (scene.cu, dota_eval.cu)
+//   iou_poly_dev       DOTA_devkit/polyiou.cpp:9-128 iou_poly in fp64 without FMA contraction (poly_nms.cu, scene.cu,
+//                      dota_eval.cu)
 //   poly_suppress_word one 64-column word of the py_cpu_nms_poly_fast suppression matrix (poly_nms.cu, scene.cu)
 //   poly_greedy_scan   the greedy keep scan over that matrix by one thread block (poly_nms.cu, scene.cu)
 #pragma once
@@ -23,6 +25,18 @@ __device__ __forceinline__ void rbox2poly_f32(float cx, float cy, float w, float
   o[6] = __fadd_rn(__fsub_rn(cx, v1x), v2x);  // point4 = center - vector1 + vector2
   o[7] = __fadd_rn(__fsub_rn(cy, v1y), v2y);
 }
+
+// Python's round(x, n) for p10 = 10^n on a double |x| * p10 < 2^52: the nearest integer to the EXACT product, ties to even
+// (py_round_int), divided by 10^n in IEEE arithmetic (the double strtod returns for the rounded decimal string).
+// x * p10 = y + e exactly; the correction applies when y is a tie but the exact product is not.
+__device__ __forceinline__ double py_round_int(double x, double p10) {
+  const double y = __dmul_rn(x, p10);
+  const double e = __fma_rn(x, p10, -y);
+  double k = rint(y);
+  if (fabs(__dsub_rn(y, k)) == 0.5 && e != 0.0) k = e > 0.0 ? __dadd_rn(y, 0.5) : __dsub_rn(y, 0.5);
+  return k;
+}
+__device__ __forceinline__ double py_round(double x, double p10) { return __ddiv_rn(py_round_int(x, p10), p10); }
 
 constexpr double PEPS = 1e-8;
 

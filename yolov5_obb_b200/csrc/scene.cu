@@ -66,18 +66,6 @@ __global__ void k_scene_tiles_s2d_u8(const uint8_t* __restrict__ scene, long lon
   }
 }
 
-// Python's round(x, n) for p10 = 10^n on a double |x| * p10 < 2^52: the nearest integer to the EXACT product, ties to even
-// (py_round_int), divided by 10^n in IEEE arithmetic (the double strtod returns for the rounded decimal string).
-// x * p10 = y + e exactly; the correction applies when y is a tie but the exact product is not.
-__device__ __forceinline__ double py_round_int(double x, double p10) {
-  const double y = __dmul_rn(x, p10);
-  const double e = __fma_rn(x, p10, -y);
-  double k = rint(y);
-  if (fabs(__dsub_rn(y, k)) == 0.5 && e != 0.0) k = e > 0.0 ? __dadd_rn(y, 0.5) : __dsub_rn(y, 0.5);
-  return k;
-}
-__device__ __forceinline__ double py_round(double x, double p10) { return __ddiv_rn(py_round_int(x, p10), p10); }
-
 constexpr int KEY_CLS_SHIFT = 57, KEY_SCORE_SHIFT = 40;
 constexpr unsigned long long KEY_SLOT_MASK = (1ull << KEY_SCORE_SHIFT) - 1;
 constexpr unsigned long long KEY_NONE = ~0ull;
