@@ -167,6 +167,7 @@ class Conv:
             d.det_no, d.det_decode, d.det_stride = det["no"], int(det["decode"]), float(det["stride"])  # decode 2 = compact records
             d.det_anchor = (c_float * 6)(*[float(v) for v in det["anchors_px"]])
         self._keep = (x, w_packed, bias_pad, out, res, out2x, det)  # buffers must outlive the descriptors
+        self.desc = d  # what the kernel was told (tests/convref.py evaluates it)
         self._h = c_void_p()
         with torch.cuda.device(x.buf.device):
             rc = _lib.lib().y5obb_conv_create(ctypes.byref(d), ctypes.byref(self._h))

@@ -149,6 +149,7 @@ class BackwardPlan:
             wg = Wgrad(dzd.data_ptr(), det.na * bn, xin.ptr, xin.pix_stride, grad_of(mi.weight), B, det.na * bn, H, W, Cin, H, W,
                        1, 1, 0, keep=(dzd, xin.buf, self.flat), param_layout=True, co_group=(det.no, bn))
             self.keep.append(wg)
+            part["wgrad"] = wg
             self.flops += 2.0 * B * H * W * det.na * bn * Cin
             add("wgrad", lambda st, wg=wg: wg.run(st))
             # dgrad: gx (+)= dz @ W  (1x1): weights [Cout'=Cin][Cin'=na*bn]
@@ -156,6 +157,7 @@ class BackwardPlan:
             part["wT"] = wT
             op, wp = add_dgrad(Slice.full(dzd), wT, 1, 0, gslice(xin), "detect dgrad")
             part["dgrad_wp"] = wp
+            part["dgrad_ops"] = [op]
             self.keep.append(op)
 
         # ---------------- conv layers, reverse ----------------
@@ -241,6 +243,7 @@ class BackwardPlan:
                 wg = Wgrad(dz.data_ptr(), Cout, x_ptr, x_ps, grad_of(conv.weight), B, Cout, Hh, Ww, Cin_w, Hi, Wi, kw_, sw_, pw_,
                            keep=(dz, x_keep, self.flat), param_layout=True)
             self.keep.append(wg)
+            part["wgrad"] = wg
             self.flops += 2.0 * npix * Cout * Cin_w * ntap
             add("wgrad", lambda st, wg=wg: wg.run(st))
 
@@ -249,9 +252,11 @@ class BackwardPlan:
                 gx = gslice(x)
                 w_d = torch.zeros((x.C, Cout, k, k), device=dev)  # filled by refresh()
                 part["w_d"] = w_d
+                part["dgrad_ops"] = []  # the conv launches that produce gx, in launch order
                 if s == 1:
                     op, wp = add_dgrad(Slice.full(dz), w_d, k, k - 1 - p, gx, "dgrad")
                     part["dgrad_wp"] = wp
+                    part["dgrad_ops"].append(op)
                     self.keep.append(op)
                 elif k == 3 and p == 1 and x.H % 2 == 0 and x.W % 2 == 0 and os.environ.get("Y5OBB_DGRAD_S2", "phase") == "phase":
                     # Output pixels of parity (ph, pw) only see the taps of matching parity: four 1- / 2-tap stride-1
@@ -270,6 +275,7 @@ class BackwardPlan:
                             self.flops += op.info()["flops"]
                             add("dgrad", lambda st, h=op._h: _lib.check(L.y5obb_conv_run(h, st), "dgrad s2 phase"))
                             part["dgrad_s2"].append((ph * 2 + pw, wp))
+                            part["dgrad_ops"].append(op)
                             self.keep.append(op)
                 else:
                     dzup = bf(B, x.H, x.W, Cout)
@@ -277,6 +283,7 @@ class BackwardPlan:
                                       _lib.check(L.y5obb_zero_stuff2x(dz.data_ptr(), C, dzup.data_ptr(), C, npix, C, W, st), "zero_stuff"))
                     op, wp = add_dgrad(Slice.full(dzup), w_d, k, k - 1 - p, gx, "dgrad s2")
                     part["dgrad_wp"] = wp
+                    part["dgrad_ops"].append(op)
                     self.keep.append(op)
         self.refresh()
 

@@ -35,6 +35,7 @@ class Wgrad:
         rows = Cout if not co_group[1] else Cout // co_group[1] * co_group[0]
         assert dw.dtype == torch.float32 and dw.is_contiguous() and dw.numel() == kh * kw * rows * Cin
         self._keep = (dw,) + tuple(keep)
+        self.desc = d  # what the kernel was told (tests/convref.py evaluates it)
         self._h = c_void_p()
         self.device = dw.device
         with torch.cuda.device(self.device):
