@@ -413,7 +413,38 @@ int y5obb_val_match_f32(const float* pred7, const int64_t* counts, int batch, in
                         const float* scale5, const float* iouv, int niou, uint8_t* correct, float* polyn8, float* hbbn4,
                         int* overflow_flag, void* stream);
 
-/* ---- float polygon NMS / rotated-box overlaps (rows A14, B4) ---------------------------------------------------------
+/* ---- validation metrics: val.py:209-276 stats + utils/metrics.py:21-114 ap_per_class (plot=False) ---------------------
+ * y5obb_val_stats_append: one asynchronous launch per batch.  Appends the valid rows of every image b (the first
+ * min(counts[b], max_det) rows of pred7 [batch, max_det, 7], including images without labels) as tp [capacity, niou]
+ * (correct [batch, max_det, niou] != 0), conf [capacity] fp32, cls [capacity] int32 and key [capacity] =
+ * (image_base + b) << 32 | row, at the running row count *n_rows (device), which it advances.  labels [n_labels,
+ * label_stride] fp32 = (image, cls, ...): the classes of the rows whose image is an integer in [0, batch) (including images
+ * without detections) are added to nt [nc] (int64).  nms_cap >= 0: counts has batch + 1 entries (non_max_suppression_obb's
+ * async form) and the batch is appended only when 0 <= counts[batch] <= nms_cap and no count is negative; otherwise nothing
+ * is appended and *skip = 1 (else 0), so that the caller re-runs the batch.  flags [3] int32, zero before the first call:
+ * flags[0] |= 1 for a detection or label class that is not an integer in [0, nc) (the row's cls is stored as -1), |= 2 for
+ * rows past capacity (not stored); flags[1] = 1 once any appended tp is set (val.py:270 stats[0].any()); flags[2] is the
+ * launch's block counter.  batch <= 4096. */
+int y5obb_val_stats_append(const float* pred7, const int64_t* counts, int batch, int max_det, int64_t nms_cap,
+                           const uint8_t* correct, int niou, const float* labels, int64_t n_labels, int label_stride,
+                           int64_t image_base, uint8_t* tp, float* conf, int32_t* cls, int64_t* key, int64_t capacity,
+                           int64_t* n_rows, int64_t* nt, int nc, int32_t* flags, int32_t* skip, void* stream);
+/* y5obb_ap_per_class_f64: ap_per_class over the first min(*n_rows, capacity) rows, bit for bit in fp64.  The row count stays
+ * on the device: every pass runs over the whole capacity and rows past the count carry sentinel keys that sort behind every
+ * class, so the call needs no host read.  Rows are ordered by descending conf with ties in ascending key (image, row) order:
+ * ordered != 0 promises that the rows were appended in key order, otherwise a radix sort by key comes first.  Classes:
+ * those with nt > 0, ascending (np.unique(target_cls)); rows of other classes are ignored.  Outputs (device, the first
+ * *n_u rows meaningful, the rest zero): ap [nc, niou] (compute_ap: 101-point np.interp of the suffix-max envelope, np.trapz
+ * in numpy's summation order), p / r [nc, 1000] (np.interp on px = np.linspace(0, 1, 1000), left = 1 / 0), ap_class [nc]
+ * int32 (-1 past *n_u), n_u [1] int32.  A class with labels but no rows gets zeros.  The 101-point interpolation assumes
+ * recall <= 1 in every column (no class has more true positives than labels), which y5obb_val_match_f32 guarantees.
+ * Requires capacity * niou <= INT_MAX; Y5OBB_EWORKSPACE when ws_bytes < y5obb_ap_per_class_workspace_bytes. */
+size_t y5obb_ap_per_class_workspace_bytes(int64_t capacity, int niou, int nc);
+int y5obb_ap_per_class_f64(const uint8_t* tp, const float* conf, const int32_t* cls, const int64_t* key, const int64_t* n_rows,
+                           int64_t capacity, int ordered, const int64_t* nt, int nc, int niou, double* ap, double* p, double* r,
+                           int32_t* ap_class, int32_t* n_u, void* ws, size_t ws_bytes, void* stream);
+
+/* ---- float polygon NMS / rotated-box overlaps (rows A14, B4)---------------------------------------------------------
  * Device-pointer forms of  utils/nms_rotated/src/nms_rotated_ext.cpp:42-55 nms_poly -> src/poly_nms_cuda.cu:144-261 (K2),
  * DOTA_devkit/poly_nms_gpu/poly_nms_kernel.cu:214-329 (K3) and poly_overlaps_kernel.cu:283-427 (K4); the float polygon IoU
  * restates the reference's expression by expression (union == 0 -> (inter + 1) / (union + 1)).

@@ -98,6 +98,12 @@ PROTOTYPES = {
                                     c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                                     c_void_p]),
     "y5obb_task1_round_f64": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
+    "y5obb_val_stats_append": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_int, c_void_p, c_int64, c_int,
+                                       c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int,
+                                       c_void_p, c_void_p, c_void_p]),
+    "y5obb_ap_per_class_workspace_bytes": (c_size_t, [c_int64, c_int, c_int]),
+    "y5obb_ap_per_class_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 SCENE_MAX_CLASS_CANDIDATES = 65536  # Y5OBB_SCENE_MAX_CLASS_CANDIDATES
