@@ -444,6 +444,53 @@ int y5obb_ap_per_class_f64(const uint8_t* tp, const float* conf, const int32_t* 
                            int64_t capacity, int ordered, const int64_t* nt, int nc, int niou, double* ap, double* p, double* r,
                            int32_t* ap_class, int32_t* n_u, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- training augmentation (utils/datasets.py:561-672, utils/augmentations.py:48-61, :131-222, :276-281) -------------
+ * Replaces LoadImagesAndLabels.__getitem__ (augment=True, rect=False, perspective == 0) + collate_fn for a batch.  The random
+ * draws and the matrices stay on the host (yolov5_obb_b200/augment.py plan_sample); a batch is B records of this layout.
+ * Placement p = 4 g + i is image i of group g: group 0 is load_mosaic's 2S mosaic (4 placements, canvas 2S) or the
+ * letterboxed image (1 placement, canvas S); group 1 is mixup's second mosaic.  A placement puts image img[p] on the canvas
+ * rectangle rect[p] = (x1a, y1a, x2a, y2a), canvas = image + pad[p]; its labels move by lpad[p] (fp32 add).  minv[g] is the
+ * inverse warpAffine computes from m[g] = M[:2] of random_perspective (fp64, row-major). */
+#define Y5OBB_AUG_MAX_PLACE 8
+#define Y5OBB_AUG_MOSAIC 1
+#define Y5OBB_AUG_MIXUP 2
+#define Y5OBB_AUG_HSV 4
+#define Y5OBB_AUG_FLIPUD 8
+#define Y5OBB_AUG_FLIPLR 16
+typedef struct {
+  int32_t img[Y5OBB_AUG_MAX_PLACE];
+  int32_t rect[4 * Y5OBB_AUG_MAX_PLACE];
+  int32_t pad[2 * Y5OBB_AUG_MAX_PLACE];
+  float lpad[2 * Y5OBB_AUG_MAX_PLACE];
+  double minv[12], m[12];
+  double mix_r, mix_1mr;     /* np.random.beta(32, 32) and 1 - r (mixup, Y5OBB_AUG_MIXUP) */
+  int32_t n_place[2], canvas[2];
+  int32_t flags, reserved;
+  uint8_t lut[768];          /* augment_hsv's hue, saturation, value LUTs (Y5OBB_AUG_HSV) */
+} y5obb_augment_sample;
+/* The dataset: images uint8 HWC BGR in one flat buffer, labels [*, 9] fp32 (cls, poly) in another; meta [n_images][5] int64 =
+ * (image byte offset, h, w, first label row, label count).
+ * y5obb_augment_check (host pointers): refuses S not a multiple of 32, images over S or outside the buffers, labels
+ * outside the label buffer, and records with bad image ids, placement counts, canvases or rectangles outside the canvas or
+ * the image.  The launch entries take device copies of meta and recs; a bad id there is skipped, never read.
+ * y5obb_augment_images_u8: out [B, 3, S, S] uint8 RGB (utils/datasets.py:662): per pixel the canvas (never materialised)
+ *   sampled by cv2.warpAffine's fixed-point INTER_LINEAR with border 114, mixup's fp64 blend truncated, augment_hsv's
+ *   COLOR_BGR2HSV / LUT / COLOR_HSV2BGR round trip (OpenCV 4.13's 8-bit arithmetic), flipud, fliplr.
+ * y5obb_augment_labels: candidates are every label of every placement in (sample, placement) order; cand_start [B*8 + 1]
+ *   is their exclusive prefix per placement (ncand = cand_start[B*8]).  Each goes through + lpad (fp32), load_mosaic's
+ *   poly_filter on the 2S canvas (fp32), xy @ M.T (fp64), poly_filter on S, the cast to fp32, the flips (S - y - 1 in fp32),
+ *   poly2rbox and labels_mask (:644-646, quirks included); survivors are compacted in order into rows [nt, tcols]:
+ *   tcols = 7 + nc_theta -> (image, cls, cx, cy, l, s, theta, CSL row of sigma csl_radius); tcols == 8 -> column 7 is
+ *   int(nc_theta / 2 - angle) (the loss's compact layout).  *nt (device) receives the count; rows needs ncand * tcols floats. */
+int y5obb_augment_check(const int64_t* meta, int n_images, int64_t images_bytes, int64_t n_labels,
+                        const y5obb_augment_sample* recs, int B, int S);
+int y5obb_augment_images_u8(const uint8_t* images, const int64_t* meta, int n_images, const y5obb_augment_sample* recs,
+                            int B, int S, uint8_t* out, void* stream);
+size_t y5obb_augment_labels_workspace_bytes(int64_t ncand);
+int y5obb_augment_labels(const float* labels, const int64_t* meta, int n_images, const y5obb_augment_sample* recs,
+                         const int64_t* cand_start, int B, int64_t ncand, int S, int nc_theta, double csl_radius, int tcols,
+                         float* rows, int64_t* nt, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- float polygon NMS / rotated-box overlaps (rows A14, B4)---------------------------------------------------------
  * Device-pointer forms of  utils/nms_rotated/src/nms_rotated_ext.cpp:42-55 nms_poly -> src/poly_nms_cuda.cu:144-261 (K2),
  * DOTA_devkit/poly_nms_gpu/poly_nms_kernel.cu:214-329 (K3) and poly_overlaps_kernel.cu:283-427 (K4); the float polygon IoU

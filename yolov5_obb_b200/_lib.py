@@ -104,6 +104,11 @@ PROTOTYPES = {
     "y5obb_ap_per_class_workspace_bytes": (c_size_t, [c_int64, c_int, c_int]),
     "y5obb_ap_per_class_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int, c_int,
                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "y5obb_augment_check": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_int, c_int]),
+    "y5obb_augment_images_u8": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "y5obb_augment_labels_workspace_bytes": (c_size_t, [c_int64]),
+    "y5obb_augment_labels": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int64, c_int, c_int,
+                                     ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 SCENE_MAX_CLASS_CANDIDATES = 65536  # Y5OBB_SCENE_MAX_CLASS_CANDIDATES
