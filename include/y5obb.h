@@ -151,6 +151,12 @@ typedef struct {
      each output-pixel parity class is a 1- or 2-tap stride-1 convolution of dz written to every other pixel. */
   int out_h, out_w;
   int64_t out_row_stride, out_img_stride, res_row_stride, res_img_stride;
+  /* optional de-scale of a test-time-augmentation branch (MODE_DETECT with det_decode 1 or 2; 0 = off): after the decode,
+     x, y, w and h are multiplied by det_inv_scale (the fp32 reciprocal of the fp32 scale, which is what ATen's `p[..., :4] /= s`
+     computes on CUDA), then x = det_flip_w - x when det_flip_w > 0 (the left-right de-flip, det_flip_w = image width);
+     _descale_pred, models/yolo.py:183-198.  The angle columns are left as they are, as the reference leaves them. */
+  int det_descale;
+  float det_inv_scale, det_flip_w;
 } y5obb_conv_desc;
 
 int y5obb_conv_tiling(int cin, int cout, int mode, int det_no, int* block_k, int* block_n, int* cin_pad,
@@ -171,6 +177,16 @@ void y5obb_conv_destroy(y5obb_conv_t* conv);
 int y5obb_stem_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream);
 /* same for a uint8 image, with the caller-side `/ 255` (train.py:299, val.py:187-188) folded in */
 int y5obb_stem_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream);
+/* y5obb_scale_img_s2d: scale_img (utils/torch_utils.py:239-249) of one test-time-augmentation branch straight into the stem
+ * input: F.interpolate(x or x.flip(3), size=(h, w), mode='bilinear', align_corners=False) with ATen's CUDA arithmetic
+ * (upsample_bilinear2d_out_frame<float, float>, its fused products restated), then F.pad right / bottom with pad_value to
+ * Hp x Wp, written in y5obb_stem_s2d's layout [B, Hp/2, Wp/2 + 2*pad_cols, 16].  x [B, 3, H, W]; flip_lr != 0 resamples
+ * x.flip(3); h <= Hp, w <= Wp, Hp and Wp even.  The pad_cols columns are not written. */
+int y5obb_scale_img_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                        int flip_lr, float pad_value, int pad_cols, void* stream);
+/* same for a uint8 image: each input value is (float)u / 255.0f, as in y5obb_stem_s2d_u8 */
+int y5obb_scale_img_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                           int flip_lr, float pad_value, int pad_cols, void* stream);
 int y5obb_sppf_pool(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream);
 
 /* ---- loss ------------------------------------------------------------------------------------

@@ -87,6 +87,8 @@ PROTOTYPES = {
     "y5obb_detect_grad_pack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_stem_s2d": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_stem_s2d_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "y5obb_scale_img_s2d": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float, c_int, c_void_p]),
+    "y5obb_scale_img_s2d_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float, c_int, c_void_p]),
     "y5obb_sppf_pool": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_scene_tiles_s2d_u8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                          c_void_p]),

@@ -30,6 +30,7 @@ class ConvDesc(ctypes.Structure):
         ("det_no", c_int), ("det_decode", c_int), ("det_stride", c_float), ("det_anchor", c_float * 6),
         ("out_h", c_int), ("out_w", c_int), ("out_row_stride", c_int64), ("out_img_stride", c_int64),
         ("res_row_stride", c_int64), ("res_img_stride", c_int64),
+        ("det_descale", c_int), ("det_inv_scale", c_float), ("det_flip_w", c_float),
     ]
 
 
@@ -166,6 +167,9 @@ class Conv:
             d.det_rows_per_image, d.det_row_off = det["rows_per_image"], det["row_off"]
             d.det_no, d.det_decode, d.det_stride = det["no"], int(det["decode"]), float(det["stride"])  # decode 2 = compact records
             d.det_anchor = (c_float * 6)(*[float(v) for v in det["anchors_px"]])
+            if det.get("descale") is not None:   # (inv_scale, flip_w): a test-time-augmentation branch (engine.TTAPlan)
+                d.det_descale = 1
+                d.det_inv_scale, d.det_flip_w = (float(v) for v in det["descale"])
         self._keep = (x, w_packed, bias_pad, out, res, out2x, det)  # buffers must outlive the descriptors
         self.desc = d  # what the kernel was told (tests/convref.py evaluates it)
         self._h = c_void_p()

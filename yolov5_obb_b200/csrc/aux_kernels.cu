@@ -6,8 +6,10 @@
 //   y5obb_sppf_pool    the three chained 5x5/s1/p2 max-pools of SPPF (models/common.py:181-196) in one
 //                      pass: y1 = 5x5, y2 = 9x9, y3 = 13x13 windows of x (max-pool composition), written
 //                      at channel offsets C, 2C, 3C of the same buffer (the torch.cat disappears).
-// Algorithmic bytes: stem_s2d reads 12*H*W fp32 and writes H*W/4 * 32 B per image; sppf_pool reads
-// H*W*C*2 and writes 3x that.
+//   y5obb_scale_img_s2d  scale_img (bilinear resample, optional lr flip, pad) of a test-time-augmentation branch into
+//                      the same stem layout.
+// Algorithmic bytes: stem_s2d reads 12*H*W fp32 and writes H*W/4 * 32 B per image; scale_img_s2d reads the input once
+// (3*H*W elements) and writes Hp*Wp/4 * 32 B per image; sppf_pool reads H*W*C*2 and writes 3x that.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -81,6 +83,95 @@ __global__ void k_stem_s2d_u8(const uint8_t* __restrict__ x, __nv_bfloat16* __re
     dst[0] = o[0];
     dst[1] = o[1];
   }
+}
+
+// scale_img (utils/torch_utils.py:239-249) of a test-time-augmentation branch, written as the stem input.  Each output pixel
+// is ATen's upsample_bilinear2d_out_frame<float, float> sample (align_corners=False), with the products its sm_90 build fuses
+// written as explicit _rn intrinsics so that the result does not depend on this build's contraction choices:
+//   src = max(fma(scale, dst + 0.5, -0.5), 0), i0 = (int)src, i1 = i0 + (i0 < in - 1), l1 = src - i0, l0 = 1 - l1,
+//   val = fma(h0l, fma(w0l, x00, w1l * x01), h1l * fma(w0l, x10, w1l * x11))
+// (the second product of each sum is the plain multiply: FMUL + FFMA pairs in the sm_90 SASS torch ships).
+// Pixels at or beyond (h, w) hold F.pad's value.  The left-right flip reads column W - 1 - xs of x.
+__device__ __forceinline__ float ld_px(const float* p, long long i) { return p[i]; }
+__device__ __forceinline__ float ld_px(const uint8_t* p, long long i) { return (float)p[i] / 255.0f; }
+
+__device__ __forceinline__ void bil_src(float scale, int dst, int in, int& i0, int& i1, float& l0, float& l1) {
+  float s = __fmaf_rn(scale, (float)dst + 0.5f, -0.5f);
+  s = s < 0.0f ? 0.0f : s;
+  i0 = (int)s;
+  i1 = i0 + (i0 < in - 1 ? 1 : 0);
+  l1 = __fsub_rn(s, (float)i0);
+  l0 = __fsub_rn(1.0f, l1);
+}
+
+template <typename T>
+__global__ void k_scale_img_s2d(const T* __restrict__ x, __nv_bfloat16* __restrict__ out, int B, int H, int W, int h, int w,
+                                int Hp, int Wp, int flip, float pad_value, float rh, float rw, int pad_cols) {
+  const int Ho = Hp >> 1, Wo = Wp >> 1;
+  const long long total = (long long)B * Ho * Wo;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int wo = (int)(i % Wo);
+    const long long r = i / Wo;
+    const int ho = (int)(r % Ho);
+    const int b = (int)(r / Ho);
+    float v[16];
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy) {
+      const int oy = 2 * ho + dy;
+      int y0, y1;
+      float hl0, hl1;
+      bil_src(rh, oy, H, y0, y1, hl0, hl1);
+#pragma unroll
+      for (int dx = 0; dx < 2; ++dx) {
+        const int ox = 2 * wo + dx;
+        float* d = v + (dy * 2 + dx) * 3;
+        if (oy >= h || ox >= w) {
+          d[0] = d[1] = d[2] = pad_value;
+          continue;
+        }
+        int x0, x1;
+        float wl0, wl1;
+        bil_src(rw, ox, W, x0, x1, wl0, wl1);
+        if (flip) {  // x.flip(3)[..., xs] = x[..., W - 1 - xs]
+          x0 = W - 1 - x0;
+          x1 = W - 1 - x1;
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const T* p = x + ((long long)b * 3 + c) * H * W;
+          const long long r0 = (long long)y0 * W, r1 = (long long)y1 * W;
+          const float a = __fmaf_rn(wl0, ld_px(p, r0 + x0), __fmul_rn(wl1, ld_px(p, r0 + x1)));
+          const float e = __fmaf_rn(wl0, ld_px(p, r1 + x0), __fmul_rn(wl1, ld_px(p, r1 + x1)));
+          d[c] = __fmaf_rn(hl0, a, __fmul_rn(hl1, e));
+        }
+      }
+    }
+    v[12] = v[13] = v[14] = v[15] = 0.f;
+    uint4 o[2];
+    __nv_bfloat162* hv = reinterpret_cast<__nv_bfloat162*>(o);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) hv[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    uint4* dst = reinterpret_cast<uint4*>(out + ((r * (Wo + 2 * pad_cols)) + wo + pad_cols) * 16);
+    dst[0] = o[0];
+    dst[1] = o[1];
+  }
+}
+
+template <typename T>
+int scale_img_s2d(const T* x, void* out, int B, int H, int W, int h, int w, int Hp, int Wp, int flip, float pad_value,
+                  int pad_cols, void* stream) {
+  if (!x || !out || B <= 0 || H <= 0 || W <= 0 || h <= 0 || w <= 0 || Hp <= 0 || Wp <= 0 || (Hp & 1) || (Wp & 1) ||
+      h > Hp || w > Wp || pad_cols < 0)
+    return Y5OBB_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(x) & (sizeof(T) - 1)) || (reinterpret_cast<uintptr_t>(out) & 15)) return Y5OBB_EINVAL;
+  // area_pixel_compute_scale (align_corners=False, no scale factor): (float)in / out, on the host as ATen does it
+  const float rh = (float)H / (float)h, rw = (float)W / (float)w;
+  const long long total = (long long)B * (Hp / 2) * (Wp / 2);
+  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
+  k_scale_img_s2d<T><<<grid, 256, 0, (cudaStream_t)stream>>>(x, static_cast<__nv_bfloat16*>(out), B, H, W, h, w, Hp, Wp,
+                                                             flip ? 1 : 0, pad_value, rh, rw, pad_cols);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
 }
 
 __device__ __forceinline__ void vmax8(uint4& a, const uint4& b) {
@@ -195,6 +286,16 @@ int y5obb_stem_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int
   k_stem_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(x_nchw, static_cast<__nv_bfloat16*>(out_nhwc16), B, H, W, pad_cols);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
+}
+
+int y5obb_scale_img_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                        int flip_lr, float pad_value, int pad_cols, void* stream) {
+  return scale_img_s2d(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
+}
+
+int y5obb_scale_img_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                           int flip_lr, float pad_value, int pad_cols, void* stream) {
+  return scale_img_s2d(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
 }
 
 int y5obb_sppf_pool(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream) {

@@ -98,6 +98,8 @@ struct ConvK {
   int det_rec_w;           // floats per compact record: (5 + nc + 1) rounded up to 4
   float det_stride;
   float det_anchor[6];
+  int det_descale;         // 1: test-time-augmentation branch, x y w h *= det_inv_scale, then x = det_flip_w - x if > 0
+  float det_inv_scale, det_flip_w;
 };
 
 struct TileCoord {
@@ -273,6 +275,12 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
             f[1] = (f[1] * 2.0f - 0.5f + (float)h) * p.det_stride;
             f[2] = (f[2] * 2.0f) * (f[2] * 2.0f) * p.det_anchor[2 * a];
             f[3] = (f[3] * 2.0f) * (f[3] * 2.0f) * p.det_anchor[2 * a + 1];
+            if (p.det_descale) {  // _descale_pred (models/yolo.py:183-198): ATen's `/= s` is a multiply by the fp32 1/s,
+                                  // the lr de-flip W - x; _rn so that neither contracts into the decode's FMAs
+#pragma unroll
+              for (int k = 0; k < 4; ++k) f[k] = __fmul_rn(f[k], p.det_inv_scale);
+              if (p.det_flip_w > 0.0f) f[0] = __fsub_rn(p.det_flip_w, f[0]);
+            }
           }
           if (p.det_decode == 2) {
 #pragma unroll
@@ -701,6 +709,13 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
   k.det_rec_w = ((d->det_no - 180 + 1) + 3) / 4 * 4;
   k.det_stride = d->det_stride;
   for (int i = 0; i < 6; ++i) k.det_anchor[i] = d->det_anchor[i];
+  k.det_descale = d->det_descale ? 1 : 0;
+  k.det_inv_scale = d->det_inv_scale;
+  k.det_flip_w = d->det_flip_w;
+  if (d->det_descale && (d->mode != MODE_DETECT || !d->det_decode || !(d->det_inv_scale > 0.0f) || d->det_flip_w < 0.0f)) {
+    delete o;
+    return Y5OBB_EINVAL;
+  }
   if (d->mode == MODE_CONV) {
     if (!d->out || d->out_pix_stride % 8 || (reinterpret_cast<uintptr_t>(d->out) & 15) || d->Cout % 8 ||
         (d->res && (d->res_pix_stride % 8 || (reinterpret_cast<uintptr_t>(d->res) & 15))) ||

@@ -15,8 +15,10 @@ Layout decisions (all NHWC bf16):
 BatchNorm is folded into the conv weights exactly as utils/torch_utils.py:192-212 (fuse_conv_and_bn).
 """
 import ctypes
+import math
 from typing import List, Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -51,7 +53,13 @@ def _is(m, name: str) -> bool:
 
 
 class InferenceEngine:
-    def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, conv_flags: int = 0, compact_detect: bool = False):
+    def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, conv_flags: int = 0, compact_detect: bool = False,
+                 det_out: Optional[torch.Tensor] = None, det_row_base: int = 0, levels=None, descale=None):
+        """The keyword options let several plans write one output (TTAPlan); their defaults give the plain plan:
+        det_out       an external [B, rows_per_image, no | rec_w] fp32 tensor the Detect epilogue writes into, from row
+                      `det_row_base` of every image on (default: an engine-owned tensor holding exactly this plan's rows);
+        levels        the Detect levels to emit (default all).  Ops whose outputs reach no kept level are not emitted;
+        descale       (inv_scale, flip_w): the Detect epilogue de-scales x y w h and de-flips x (y5obb_conv_desc.det_descale)."""
         device = torch.device(device)
         if device.type != "cuda":
             raise RuntimeError("InferenceEngine needs a CUDA device (sm_90a); there is no CPU path")
@@ -96,6 +104,17 @@ class InferenceEngine:
             elif _is(m, "Concat"):
                 ch[i], hw[i] = sum(ch[f] for f in fs), in_hw
                 assert all(hw[f] == in_hw for f in fs)
+
+        # ---- liveness: backwards from the inputs of the kept Detect levels (a pruned level's head is not emitted)
+        self.levels = tuple(range(det.nl)) if levels is None else tuple(sorted(set(int(l) for l in levels)))
+        if not self.levels or not all(0 <= l < det.nl for l in self.levels):
+            raise RuntimeError(f"Detect levels {levels} are not a non-empty subset of 0..{det.nl - 1}")
+        live = [False] * n
+        need = {det.f[l] for l in self.levels}
+        for m in reversed(layers[:-1]):
+            if m.i in need:
+                live[m.i] = True
+                need.update(src_of(m.i, f) for f in ([m.f] if isinstance(m.f, int) else m.f))
 
         arena = {"buf": None, "used": 0}
 
@@ -167,16 +186,22 @@ class InferenceEngine:
             self.hbm_bytes += info["hbm_bytes"]
             h = op._h
             self.ops.append(lambda st, h=h: L.y5obb_conv_run(h, st))
+            self.op_layers.append(cur[0])
 
         # ---- pass 3: emit ops
         # space-to-depth image with one zero pixel of padding left and right of every row: the stem's three
         # horizontal taps are then 48 CONTIGUOUS channels of an overlapping-window view (pixel stride 16)
         self.x_s2d = torch.zeros((B, H // 2, W // 2 + 2, 16), dtype=torch.bfloat16, device=device)
         self.keep.append(self.x_s2d)
+        self.op_layers = []    # per op: the top-level layer index it belongs to, ("Detect", level) for the head convs
+        cur = [None]
         for m in layers:
             i = m.i
             if _is(m, "Detect"):
                 break
+            if not live[i]:
+                continue
+            cur[0] = i
             fs = [src_of(i, f) for f in ([m.f] if isinstance(m.f, int) else m.f)]
             if _is(m, "Conv"):
                 w, b = _conv_params(m)
@@ -230,6 +255,7 @@ class InferenceEngine:
                 hh, ww = hw[i]
                 ptr, ps = cat4.data_ptr(), cat4.shape[3]
                 self.ops.append(lambda st, ptr=ptr, ps=ps, hh=hh, ww=ww, c_=c_: L.y5obb_sppf_pool(ptr, ps, B, hh, ww, c_, st))
+                self.op_layers.append(i)
                 self.hbm_bytes += 2.0 * B * hh * ww * c_ * 4
                 w2, b2 = _conv_params(m.cv2)
                 add_conv(Slice.full(cat4), w2, b2, 1, 1, 0, True, out[i])
@@ -237,24 +263,37 @@ class InferenceEngine:
 
         # ---- Detect
         self.no, self.na = det.no, det.na
-        rows = [det.na * hw[f][0] * hw[f][1] for f in det.f]
+        rows = [det.na * hw[det.f[l]][0] * hw[det.f[l]][1] for l in self.levels]
         self.rows_total = sum(rows)
         # compact_detect: the Detect epilogue writes (cx, cy, w, h, obj, cls[nc], theta index) records - all that
         # non_max_suppression_obb reads of a row - instead of the [B, A, no] tensor (96 B instead of 800 B per anchor row)
         self.compact_detect = bool(compact_detect)
         self.rec_w = ((det.nc + 6) + 3) // 4 * 4
         self.nc = det.nc
-        self.pred = torch.empty((B, self.rows_total, self.rec_w if compact_detect else det.no), dtype=torch.float32, device=device)
-        row_off = 0
-        for l, f in enumerate(det.f):
+        width = self.rec_w if compact_detect else det.no
+        if det_out is None:
+            if det_row_base:
+                raise RuntimeError("det_row_base needs an external det_out")
+            self.pred = torch.empty((B, self.rows_total, width), dtype=torch.float32, device=device)
+        else:
+            _lib.require_cuda(det_out, "det_out")
+            if (det_out.dtype != torch.float32 or not det_out.is_contiguous() or det_out.dim() != 3 or det_out.shape[0] != B
+                    or det_out.shape[2] != width or det_out.device != device or det_row_base < 0
+                    or det_row_base + self.rows_total > det_out.shape[1]):
+                raise RuntimeError(f"det_out must be a contiguous fp32 [{B}, >= {det_row_base + self.rows_total}, {width}] "
+                                   f"tensor on {device}, got {tuple(det_out.shape)} {det_out.dtype}")
+            self.pred = det_out
+        row_off = int(det_row_base)
+        for l, f in ((l, det.f[l]) for l in self.levels):
+            cur[0] = ("Detect", l)
             mi = det.m[l]
             stride = float(det.stride[l])
             anchors_px = (det.anchors[l].detach().float().cpu() * stride).flatten().tolist()
             add_conv(out[f], mi.weight.detach().float().cpu(), mi.bias.detach().float().cpu(), 1, 1, 0, False,
-                     detd=dict(out=self.pred, rows_per_image=self.rows_total, row_off=row_off, no=det.no,
+                     detd=dict(out=self.pred, rows_per_image=self.pred.shape[1], row_off=row_off, no=det.no,
                                decode=2 if compact_detect else True,
-                               stride=stride, anchors_px=anchors_px))
-            row_off += rows[l]
+                               stride=stride, anchors_px=anchors_px, descale=descale))
+            row_off += det.na * hw[f][0] * hw[f][1]
         self.hbm_bytes += 4.0 * B * self.rows_total * det.no + 4.0 * B * 3 * H * W + 2.0 * self.x_s2d.numel()
         self.n_launches = len(self.ops) + 1
 
@@ -304,3 +343,93 @@ class InferenceEngine:
             rc = op(st)
             if rc:
                 _lib.check(rc, "engine op")
+
+
+# ---- test-time augmentation (models/yolo.py:149-209 _forward_augment)
+TTA_SCALES = (1, 0.83, 0.67)   # yolo.py:151
+TTA_FLIPS = (None, 3, None)    # 3 = left-right (x.flip(3))
+TTA_PAD = 0.447                # scale_img's F.pad value (utils/torch_utils.py:249)
+
+
+def tta_geometry(H: int, W: int, gs: int = 32, nl: int = 3, na: int = 3, strides=(8, 16, 32)):
+    """Host geometry of _forward_augment for an H x W input (multiples of gs): per branch the scale and flip, scale_img's
+    resampled size (h, w) and padded size (Hp, Wp) in its own Python float arithmetic, the Detect levels _clip_augmented keeps
+    (the first branch loses its last level, the last branch its first one: for gs-multiple shapes its `shape[1] // g * 4**k`
+    row counts are exactly those levels), the branch's rows per image, its first row in the concatenated output, and the
+    de-scale constants (the fp32 reciprocal of the fp32 scale, ATen's `/= s` on CUDA; the de-flip width, 0 = none).
+    Returns (branches, rows_per_image)."""
+    if H % gs or W % gs or H <= 0 or W <= 0:
+        raise RuntimeError(f"test-time augmentation needs an image size that is a multiple of {gs}, got {H}x{W}")
+    branches, row = [], 0
+    last = len(TTA_SCALES) - 1
+    for k, (s, fl) in enumerate(zip(TTA_SCALES, TTA_FLIPS)):
+        if s == 1.0:
+            h, w, Hp, Wp = H, W, H, W
+        else:
+            h, w = int(H * s), int(W * s)
+            Hp, Wp = (math.ceil(v * s / gs) * gs for v in (H, W))
+        levels = list(range(nl))
+        if k == 0:
+            levels = levels[:-1]
+        if k == last:
+            levels = levels[1:]
+        level_rows = [na * (Hp // st) * (Wp // st) for st in strides]
+        rows = sum(level_rows[l] for l in levels)
+        branches.append(dict(scale=s, flip=fl, h=h, w=w, Hp=Hp, Wp=Wp, levels=tuple(levels), level_rows=level_rows,
+                             row_off=row, rows=rows, inv_scale=float(np.float32(1.0) / np.float32(s)),
+                             flip_w=float(W) if fl == 3 else 0.0))
+        row += rows
+    return branches, row
+
+
+class TTAPlan:
+    """_forward_augment on the device: three InferenceEngines (one per scale) whose Detect epilogues de-scale their rows and
+    write them into one shared [B, rows_total, no] (or compact-record) tensor at the branch's row offset, so that the
+    torch.cat of the clipped branches is never formed.  Branch 0 runs the plain stem layout pass; branches 1 and 2 resample
+    the input into their stem buffer (y5obb_scale_img_s2d) and run forward_s2d().  Every plan skips the ops that feed only the
+    Detect level _clip_augmented drops.  All work is on the current stream; each engine replays its own CUDA graph."""
+
+    def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, compact_detect: bool = False, conv_flags: int = 0):
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("TTAPlan needs a CUDA device (sm_90a); there is no CPU path")
+        det = model.model[-1]
+        self.branches, self.rows_total = tta_geometry(H, W, int(max(model.stride)), det.nl, det.na,
+                                                      [int(s) for s in det.stride])
+        self.device, self.B, self.H, self.W = device, B, H, W
+        self.nc, self.no = det.nc, det.no
+        self.rec_w = ((det.nc + 6) + 3) // 4 * 4
+        self.compact_detect = bool(compact_detect)
+        self.pred = torch.empty((B, self.rows_total, self.rec_w if compact_detect else det.no), dtype=torch.float32,
+                                device=device)
+        self.engines = [InferenceEngine(model, B, g["Hp"], g["Wp"], device, conv_flags, compact_detect, det_out=self.pred,
+                                        det_row_base=g["row_off"], levels=g["levels"],
+                                        descale=None if g["scale"] == 1 else (g["inv_scale"], g["flip_w"]))
+                        for g in self.branches]
+        self.flops = sum(e.flops for e in self.engines)
+
+    def resample_bytes(self, k: int, itemsize: int = 4) -> float:
+        """Algorithmic bytes of branch k's resample: one read of the input plus the stem-layout output."""
+        g = self.branches[k]
+        return float(self.B) * (3 * self.H * self.W * itemsize + (g["Hp"] // 2) * (g["Wp"] // 2) * 32)
+
+    def resample(self, x: torch.Tensor, k: int) -> None:
+        """scale_img of branch k (k >= 1) into that engine's x_s2d."""
+        g, e = self.branches[k], self.engines[k]
+        fn = _lib.lib().y5obb_scale_img_s2d_u8 if x.dtype == torch.uint8 else _lib.lib().y5obb_scale_img_s2d
+        _lib.check(fn(x.data_ptr(), e.x_s2d.data_ptr(), self.B, self.H, self.W, g["h"], g["w"], g["Hp"], g["Wp"],
+                      1 if g["flip"] == 3 else 0, TTA_PAD, 1, _lib.stream_ptr(self.device)), "y5obb_scale_img_s2d")
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        """x: [B,3,H,W] fp32 in [0,1] (or uint8 0..255) on this plan's device -> [B, rows_total, no] fp32 (or the compact
+        records), plan-owned, overwritten by the next call."""
+        _lib.require_cuda(x, "x")
+        if tuple(x.shape) != (self.B, 3, self.H, self.W):
+            raise RuntimeError(f"TTA plan was built for {(self.B, 3, self.H, self.W)}, got {tuple(x.shape)}")
+        x = x.contiguous() if x.dtype == torch.uint8 else x.contiguous().float()
+        with torch.cuda.device(self.device):
+            self.engines[0].forward(x)
+            for k in range(1, len(self.engines)):
+                self.resample(x, k)
+                self.engines[k].forward_s2d()
+        return self.pred

@@ -225,8 +225,10 @@ class Validator:
     read.  A batch whose NMS candidates overflowed the optimistic capacity is not appended; its skip flag is read one batch
     late, while the next batch computes, and the batch is then re-run with the blocking NMS from its device copy."""
 
-    def __init__(self, model, conf_thres: float = 0.01, iou_thres: float = 0.4, max_det: int = 1500, iouv=None):
+    def __init__(self, model, conf_thres: float = 0.01, iou_thres: float = 0.4, max_det: int = 1500, iouv=None,
+                 augment: bool = False):
         self.model = model
+        self.augment = bool(augment)   # val.py --augment: test-time augmentation (Model.detect_records(augment=True))
         self.device = _resolve(next(model.parameters()).device)
         if self.device.type != "cuda":
             raise RuntimeError("Validator needs the model on a CUDA device; there is no CPU path")
@@ -252,7 +254,8 @@ class Validator:
         from .general import non_max_suppression_obb
         x, t = _upload(im, self.device), _upload(targets.float(), self.device)
         base = stats.seen
-        dets, counts, cap = non_max_suppression_obb(self.model.detect_records(x), return_packed="async", **self.nms)
+        dets, counts, cap = non_max_suppression_obb(self.model.detect_records(x, augment=self.augment), return_packed="async",
+                                                    **self.nms)
         correct, _, _ = match_batch(dets, counts, t, shapes, self.iouv, want_geometry=False)
         skip = stats.add(dets, counts, correct, t, nms_cap=cap)
         host = torch.empty(1, dtype=torch.int32).pin_memory()
@@ -268,7 +271,7 @@ class Validator:
         if int(host[0]) == 0:
             return
         self.reruns += 1
-        dets, rows = non_max_suppression_obb(self.model.detect_records(x), return_packed=True, **self.nms)
+        dets, rows = non_max_suppression_obb(self.model.detect_records(x, augment=self.augment), return_packed=True, **self.nms)
         counts = torch.tensor(rows, dtype=torch.int64).to(self.device)
         correct, _, _ = match_batch(dets, counts, t, shapes, self.iouv, want_geometry=False)
         stats.add(dets, counts, correct, t, image_base=base)

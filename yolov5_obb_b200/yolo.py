@@ -319,15 +319,43 @@ class Model(nn.Module):
             eng._weights_sig = sig
         return eng.forward(x), None
 
-    def detect_records(self, x, slot: int = 0):
+    def forward_augment(self, x):
+        """models/yolo.py:149-161 _forward_augment on the device (test-time augmentation, `val.py --augment`,
+        `detect.py --augment`): x [B, 3, H, W] fp32 in [0, 1] or uint8, H and W multiples of 32 -> (pred [B, A_tta, nc+185]
+        fp32, None), the clipped, de-scaled rows of the scales 1, 0.83 (left-right flipped) and 0.67 in branch order
+        (plan-owned buffer, overwritten by the next call).  The angle columns of the flipped branch are not mirrored, as in
+        the reference."""
+        return self.tta_plan(tuple(x.shape), x.device).forward(x), None
+
+    def tta_plan(self, shape, device, compact_detect: bool = False, slot: int = 0):
+        """The engine.TTAPlan behind forward_augment / detect_records(augment=True) for inputs of `shape` on `device`,
+        re-planned when the weights changed since it was built."""
+        if self.training:
+            raise RuntimeError("test-time augmentation is an inference entry point (model.eval())")
+        from .engine import TTAPlan
+        device = torch.device(device)
+        key = ("tta", tuple(shape), device.index, bool(compact_detect)) + ((int(slot),) if slot else ())
+        plan = self._engines.get(key)
+        sig = self._weights_signature()
+        if plan is None or plan._weights_sig != sig:
+            self._engines.pop(key, None)   # (frees the stale plan's buffers before the new one allocates)
+            plan = self._engines[key] = TTAPlan(self, shape[0], shape[2], shape[3], device, compact_detect=compact_detect)
+            plan._weights_sig = sig
+        return plan
+
+    def detect_records(self, x, slot: int = 0, augment: bool = False):
         """Eval-mode forward for the fused post-process: instead of the [B, A, nc+185] tensor the Detect epilogue writes, per
         anchor row, the compact record (cx, cy, w, h, obj, cls[nc], theta index) - everything non_max_suppression_obb reads
         (utils/general.py:781-832) - so 96 B instead of 800 B per row cross HBM, once instead of three times.  Returns a
         general.DetectRecords, accepted by yolov5_obb_b200.general.non_max_suppression_obb in place of the prediction
         tensor (bit-identical detections: same sigmoid / decode arithmetic, same first-maximum theta rule).
         `slot` selects one of several independent plans of the same shape (own activation and record buffers, own captured
-        graph): batches in flight on DIFFERENT streams must use different slots (pipeline.DetectPipeline does)."""
+        graph): batches in flight on DIFFERENT streams must use different slots (pipeline.DetectPipeline does).
+        augment=True: the records of forward_augment's rows (test-time augmentation)."""
         from .general import DetectRecords
+        if augment:
+            plan = self.tta_plan(tuple(x.shape), x.device, compact_detect=True, slot=slot)
+            return DetectRecords(plan.forward(x), plan.nc)
         eng = self.records_plan(tuple(x.shape), x.device, slot)
         return DetectRecords(eng.forward(x), eng.nc)
 
