@@ -224,6 +224,27 @@ int y5obb_loss_forward(const y5obb_loss_desc* desc, float* loss1, float* items4,
 int y5obb_loss_backward(const y5obb_loss_desc* desc, const float* grad_loss, void* workspace,
                         size_t workspace_bytes, void* stream);
 
+/* The validation loss of val.py:198-199 (compute_loss(train_out)[1] for an eval forward; utils/loss.py:122-192) without the
+ * materialised head output: the logits the loss reads are computed from the Detect inputs.  Per level, the na obj logits of
+ * every cell (an N = na GEMM reading each feature once) and the no logits of every matched row (a gathered GEMV), accumulated
+ * in fp32 as bias + sum_c feat * w; everything after that (matching, CIoU, class / theta BCE, obj BCE, reductions) is
+ * y5obb_loss_forward's own code, so loss1 / items4 are bit-identical to y5obb_loss_forward on logits equal to these.
+ * desc.p and desc.grad are ignored and desc.H / desc.W are replaced by the feature shapes.  Forward only.
+ * Y5OBB_EINVAL when a pointer is null, C % 8 != 0, a stride is smaller than the extent it spans or not a multiple of 8
+ * elements, or feat / w is not 16-byte aligned.  The workspace holds the obj logits (4 bytes per cell) and
+ * nl * 5 * na * nt rows of no floats besides y5obb_loss_forward's own. */
+typedef struct {
+  const void* feat[3];                   /* bf16 NHWC Detect input of level i (Detect.f[i]'s output) */
+  int64_t pix_stride[3], row_stride[3], img_stride[3];  /* element strides of pixels, rows and images */
+  int H[3], W[3], C[3];                  /* feature shape; C % 8 == 0 */
+  const void* w[3];                      /* bf16 [na * no, C]: Detect.m[i].weight */
+  const float* bias[3];                  /* fp32 [na * no]:    Detect.m[i].bias */
+} y5obb_loss_head;
+
+size_t y5obb_loss_head_workspace_bytes(const y5obb_loss_desc* desc, const y5obb_loss_head* head);
+int y5obb_loss_forward_head(const y5obb_loss_desc* desc, const y5obb_loss_head* head, float* loss1, float* items4,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- post-NMS geometry and CSL targets (one thread per box, fp32, separately rounded ops) -------
  * rbox2poly: utils/rboxs_utils.py:106-126 — [n,5] (cx,cy,l,s,theta) -> [n,8] corner coordinates.
  * poly2hbb:  utils/rboxs_utils.py:147-165 — [n,8] -> [n,4] (xc, yc, w, h) of the axis-aligned hull.

@@ -13,11 +13,15 @@
 //               per-block partial sums
 //   k_final     fixed-order reductions, per-level means, gains (:185-189): loss[1], items[4]
 //   k_bwd_obj / k_bwd_rows   dL/dp written once: zeros + obj channel for every cell, then the matched rows
+// The validation loss (val.py:198-199, y5obb_loss_forward_head) reads no materialised head output: k_head_obj computes the obj
+// logits of every cell and k_head_rows the logits of the matched rows from the Detect inputs, into the workspace, and k_rows /
+// k_obj read them there (LossK.rows / .obj); everything else is the code above.
 // HBM-bound: forward reads one float per cell (32-byte sectors) + 800 bytes per matched row; backward must
 // write the dense gradient the autograd contract asks for (B * 64512 * 200 * 4 bytes at 1024x1024).
 // Everything is fp32; sums are reduced in a fixed order (deterministic), except gradient accumulation on
 // duplicate cells (atomicAdd, order-dependent in the last bit).
 #include <cub/device/device_scan.cuh>
+#include <cuda_bf16.h>
 
 #include <algorithm>
 #include <cstring>
@@ -63,6 +67,19 @@ struct LossK {
   // fp64 like the reference), 2 = the index is derived here from theta (column 6, fp32).  Modes 1/2 read gauss[].
   int csl_mode;
   float gauss[180];   // (float)exp(-(j - 90)^2 / (2 sigma^2)), j = 0..179: the un-rotated row of gaussian_label_cpu
+  // Where k_rows and k_obj read the logits.  A matched row's no logits start at
+  // rows[lvl] + cell_local * row_cell_stride + rank * row_rank_stride; cell i's obj logit is obj[lvl][i * obj_stride + obj_col].
+  // The materialised head gives (p, no, 0) and (p, no, 4); the Detect-input path gives its workspace buffers (0, no) and (1, 0).
+  const float* rows[3];
+  long long row_cell_stride, row_rank_stride;
+  const float* obj[3];
+  long long obj_stride;
+  int obj_col;
+  void* scan_tmp;
+  size_t scan_bytes;
+  // Detect-input path (y5obb_loss_forward_head): obj logits [cells] and matched-row logits [ncand, no]
+  float* head_obj;
+  float* head_rows;
 };
 
 // element c of target t's CSL row: gaussian_label_cpu's np.concatenate([y_sig[index:], y_sig[:index]]) = y_sig[(c + index) mod 180]
@@ -259,7 +276,7 @@ __global__ void k_rows(LossK L) {
   const int rank = L.rank[q];
   const RowGeom r = row_geom(L, q);
   if (r.b < 0 || r.b >= L.B) return;  // malformed target row
-  const float* ps = L.p[r.lvl] + (long long)r.cell_local * L.no;
+  const float* ps = L.rows[r.lvl] + (long long)r.cell_local * L.row_cell_stride + (long long)rank * L.row_rank_stride;
   const float* csl = L.targets + (long long)r.t * L.tcols + 7;
   const int csl_i = L.csl_mode ? csl_index(L, r.t) : 0;
   float s_cls = 0.f, s_th = 0.f;
@@ -288,7 +305,7 @@ __global__ void __launch_bounds__(OBJ_THREADS) k_obj(LossK L, int lvl) {
   const long long i = (long long)blockIdx.x * OBJ_THREADS + threadIdx.x;
   float v = 0.f;
   if (i < cells) {
-    const float x = L.p[lvl][i * L.no + 4];
+    const float x = L.obj[lvl][i * L.obj_stride + L.obj_col];
     const int w = L.winner[L.cell_off[lvl] + i];
     const float t = w >= 0 ? fmaxf(L.row_iou[w], 0.f) : 0.f;  // gr = 1.0 (:157-159)
     v = bce_logits(x, t, L.obj_pw);
@@ -301,6 +318,110 @@ __global__ void __launch_bounds__(OBJ_THREADS) k_obj(LossK L, int lvl) {
     __syncthreads();
   }
   if (threadIdx.x == 0) L.obj_partial[L.obj_block_off[lvl] + blockIdx.x] = (double)red[0];
+}
+
+// ---- Detect-input logit source (y5obb_loss_forward_head): the logits the loss reads, computed from the Detect inputs instead of
+// being read from a materialised [B, na, H, W, no] head output
+struct HeadLevel {
+  const __nv_bfloat16* feat;  // NHWC, element strides below
+  long long pix, row, img;
+  int C;
+  const __nv_bfloat16* w;     // [na * no, C]
+  const float* bias;          // [na * no]
+};
+struct HeadK {
+  HeadLevel lv[3];
+};
+
+// 8 bf16 products of two 16-byte vectors, accumulated in order into acc
+__device__ __forceinline__ float dot8(const uint4& x, const uint4& y, float acc) {
+  const __nv_bfloat162* a = reinterpret_cast<const __nv_bfloat162*>(&x);
+  const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&y);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 u = __bfloat1622float2(a[i]), v = __bfloat1622float2(b[i]);
+    acc = fmaf(u.x, v.x, acc);
+    acc = fmaf(u.y, v.y, acc);
+  }
+  return acc;
+}
+
+// obj logits of one level: head_obj[cell_off + ((b * na + a) * H + y) * W + x] = bias[a*no+4] + sum_c feat[b,y,x,c] w[a*no+4, c].
+// An N = na GEMM bound by the feature read: G lanes (a power of two dividing C/8) share a pixel, every feature byte is read once
+// with 16-byte loads, the na weight rows sit in shared memory.
+__global__ void __launch_bounds__(256) k_head_obj(LossK L, HeadLevel h, int lvl, int G) {
+  extern __shared__ uint4 s_w[];  // [na][C / 8]
+  const int C8 = h.C / 8;
+  for (int i = threadIdx.x; i < L.na * C8; i += blockDim.x) {
+    const int a = i / C8;
+    s_w[i] = *reinterpret_cast<const uint4*>(h.w + (long long)(a * L.no + 4) * h.C + (i - a * C8) * 8);
+  }
+  __syncthreads();
+  const int H = L.H[lvl], W = L.W[lvl];
+  const long long pixels = (long long)L.B * H * W;
+  const int lane = threadIdx.x & 31, g = lane & (G - 1);
+  float* out = L.head_obj + L.cell_off[lvl];
+  // warp-uniform trip count: every lane reaches the shuffles
+  const long long step = (long long)gridDim.x * blockDim.x / G;
+  for (long long base = ((long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31)) / G; base < pixels; base += step) {
+    const long long pix = base + lane / G;
+    const bool valid = pix < pixels;
+    float acc[3] = {0.f, 0.f, 0.f};
+    int b = 0, y = 0, x = 0;
+    if (valid) {
+      b = (int)(pix / ((long long)H * W));
+      const int rem = (int)(pix - (long long)b * H * W);
+      y = rem / W;
+      x = rem - y * W;
+      const __nv_bfloat16* f = h.feat + b * h.img + y * h.row + x * h.pix;
+      for (int c8 = g; c8 < C8; c8 += G) {
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(f + c8 * 8));
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+          if (a < L.na) acc[a] = dot8(v, s_w[a * C8 + c8], acc[a]);
+      }
+    }
+    for (int o = G >> 1; o; o >>= 1) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) acc[a] += __shfl_xor_sync(0xffffffffu, acc[a], o);
+    }
+    if (valid && g == 0) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+        if (a < L.na) out[(((long long)b * L.na + a) * H + y) * W + x] = h.bias[a * L.no + 4] + acc[a];
+    }
+  }
+}
+
+// the no logits of every matched row (after k_match and the scan): a gathered GEMV per row, one warp per candidate, written to
+// head_rows[rank * no + j] = bias[a*no+j] + sum_c feat[b,gj,gi,c] w[a*no+j, c]
+__global__ void k_head_rows(LossK L, HeadK hk) {
+  const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (q >= L.ncand || !L.flag[q]) return;
+  const RowGeom r = row_geom(L, q);
+  if (r.b < 0 || r.b >= L.B) return;  // k_rows skips the row too
+  const HeadLevel& h = hk.lv[r.lvl];
+  const int C8 = h.C / 8;
+  const __nv_bfloat16* f = h.feat + r.b * h.img + r.gj * h.row + r.gi * h.pix;
+  const __nv_bfloat16* w = h.w + (long long)r.a * L.no * h.C;
+  const float* bias = h.bias + r.a * L.no;
+  float* out = L.head_rows + (long long)L.rank[q] * L.no;
+  for (int j0 = 0; j0 < L.no; j0 += 4) {  // no % 4 == 0 (fill)
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int c8 = lane; c8 < C8; c8 += 32) {
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(f + c8 * 8));
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        acc[k] = dot8(v, __ldg(reinterpret_cast<const uint4*>(w + (long long)(j0 + k) * h.C + c8 * 8)), acc[k]);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
+    }
+    if (lane < 4) out[j0 + lane] = bias[j0 + lane] + (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]);
+  }
 }
 
 // one block; every sum runs in a fixed order
@@ -394,7 +515,7 @@ __global__ void k_bwd_rows(LossK L, const float* __restrict__ gloss) {
   }
 }
 
-int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* need) {
+int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* need, bool head = false) {
   if (!d || d->nl < 1 || d->nl > 3 || d->B < 1 || d->na < 1 || d->na > 3 || d->nt < 0) return Y5OBB_EINVAL;
   if (d->no != d->nc + 5 + 180 || d->no % 4) return Y5OBB_EINVAL;
   if (d->tcols != 7 && d->tcols != 8 && d->tcols < 7 + 180) return Y5OBB_EINVAL;
@@ -441,6 +562,10 @@ int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* 
     blocks += L.obj_blocks[i];
   }
   L.cell_off[d->nl] = cells;
+  for (int i = 0; i < d->nl; ++i) L.rows[i] = L.obj[i] = d->p[i];
+  L.row_cell_stride = L.obj_stride = d->no;
+  L.row_rank_stride = 0;
+  L.obj_col = 4;
   L.obj_block_off[d->nl] = blocks;
   for (int i = 0; i < 18; ++i) L.anchors[i] = d->anchors[i];
   L.ncand = d->nl * NOFF * d->na * d->nt;
@@ -460,9 +585,84 @@ int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* 
     (void)cudaGetLastError();
     scan_bytes = (1u << 20);
   }
-  c.take<char>(scan_bytes);
+  L.scan_tmp = c.take<char>(scan_bytes);
+  L.scan_bytes = scan_bytes;
+  if (head) {
+    L.head_obj = c.take<float>(cells);
+    L.head_rows = c.take<float>((size_t)nc1 * d->no);
+    for (int i = 0; i < d->nl; ++i) {
+      L.rows[i] = L.head_rows;
+      L.obj[i] = L.head_obj + L.cell_off[i];
+    }
+    L.row_cell_stride = 0;
+    L.row_rank_stride = d->no;
+    L.obj_stride = 1;
+    L.obj_col = 0;
+  }
   *need = c.used() + 256;
   if (ws && *need > ws_bytes) return Y5OBB_EWORKSPACE;
+  return Y5OBB_OK;
+}
+
+// The forward shared by both logit sources; hk != nullptr computes the logits from the Detect inputs first.
+int forward(LossK& L, const HeadK* hk, float* loss1, float* items4, cudaStream_t st) {
+  if (L.nt > 0 && !L.targets) return Y5OBB_EINVAL;
+  Y5_CUDA(cudaMemsetAsync(L.winner, 0xFF, (size_t)L.cell_off[L.nl] * sizeof(int), st));
+  if (L.ncand > 0) {
+    k_match<<<(L.ncand + 255) / 256, 256, 0, st>>>(L);
+    Y5_LAUNCH_CHECK();
+    Y5_CUDA(cub::DeviceScan::ExclusiveSum(L.scan_tmp, L.scan_bytes, L.flag, L.rank, L.ncand, st));
+    const long long threads = (long long)L.ncand * 32;
+    if (hk) {
+      k_head_rows<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(L, *hk);
+      Y5_LAUNCH_CHECK();
+    }
+    k_rows<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(L);
+    Y5_LAUNCH_CHECK();
+  } else {
+    // no targets: rank/flag single dummy entry = 0 so that level_rows() == 0
+    Y5_CUDA(cudaMemsetAsync(L.flag, 0, sizeof(int), st));
+    Y5_CUDA(cudaMemsetAsync(L.rank, 0, sizeof(int), st));
+  }
+  for (int lvl = 0; lvl < L.nl; ++lvl) {
+    if (hk) {
+      const HeadLevel& h = hk->lv[lvl];
+      const int C8 = h.C / 8;
+      int G = 1;
+      while (G < 32 && C8 % (2 * G) == 0) G *= 2;
+      const long long threads = (long long)L.B * L.H[lvl] * L.W[lvl] * G;
+      const int grid = (int)std::min<long long>((threads + 255) / 256, (long long)sm_count() * 8);
+      k_head_obj<<<grid, 256, (size_t)L.na * C8 * sizeof(uint4), st>>>(L, h, lvl, G);
+      Y5_LAUNCH_CHECK();
+    }
+    k_obj<<<L.obj_blocks[lvl], OBJ_THREADS, 0, st>>>(L, lvl);
+    Y5_LAUNCH_CHECK();
+  }
+  if (L.ncand == 0) L.ncand = 1;  // k_final reads rank[ncand-1] + flag[ncand-1]
+  k_final<<<1, 256, 0, st>>>(L, loss1, items4);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+// Checks the Detect inputs and gives the loss description they imply: H / W from the features, no materialised logits.
+int head_desc(const y5obb_loss_desc* d, const y5obb_loss_head* h, y5obb_loss_desc* dd, HeadK* hk) {
+  if (!d || !h || d->nl < 1 || d->nl > 3 || d->na < 1 || d->na > 3 || d->no < 1) return Y5OBB_EINVAL;
+  *dd = *d;
+  memset(hk, 0, sizeof(*hk));
+  for (int i = 0; i < d->nl; ++i) {
+    const int C = h->C[i], H = h->H[i], W = h->W[i];
+    const long long pix = h->pix_stride[i], row = h->row_stride[i], img = h->img_stride[i];
+    if (!h->feat[i] || !h->w[i] || !h->bias[i]) return Y5OBB_EINVAL;
+    if (C < 8 || C % 8 || H < 1 || W < 1) return Y5OBB_EINVAL;
+    if (pix < C || pix % 8 || row < (long long)W * pix || row % 8 || img < (long long)H * row || img % 8) return Y5OBB_EINVAL;
+    if ((reinterpret_cast<uintptr_t>(h->feat[i]) | reinterpret_cast<uintptr_t>(h->w[i])) & 15) return Y5OBB_EINVAL;
+    dd->p[i] = nullptr;
+    dd->grad[i] = nullptr;
+    dd->H[i] = H;
+    dd->W[i] = W;
+    hk->lv[i] = HeadLevel{reinterpret_cast<const __nv_bfloat16*>(h->feat[i]), pix, row, img, C,
+                          reinterpret_cast<const __nv_bfloat16*>(h->w[i]), h->bias[i]};
+  }
   return Y5OBB_OK;
 }
 
@@ -489,42 +689,30 @@ int y5obb_loss_forward(const y5obb_loss_desc* d, float* loss1, float* items4, vo
   if (rc) return rc;
   for (int i = 0; i < L.nl; ++i)
     if (!L.p[i]) return Y5OBB_EINVAL;
-  if (L.nt > 0 && !L.targets) return Y5OBB_EINVAL;
-  cudaStream_t st = (cudaStream_t)stream;
-  Y5_CUDA(cudaMemsetAsync(L.winner, 0xFF, (size_t)L.cell_off[L.nl] * sizeof(int), st));
-  if (L.ncand > 0) {
-    k_match<<<(L.ncand + 255) / 256, 256, 0, st>>>(L);
-    Y5_LAUNCH_CHECK();
-    // scan temp storage sits right after obj_partial in the carve order
-    Carver c(workspace);
-    c.take<int>(L.ncand);
-    c.take<int>(L.ncand);
-    c.take<int>(L.cell_off[L.nl]);
-    c.take<float>(L.ncand);
-    c.take<float>(L.ncand);
-    c.take<float>(L.ncand);
-    c.take<float>(L.ncand);
-    c.take<double>(L.obj_block_off[L.nl]);
-    size_t scan_bytes = 0;
-    Y5_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, L.flag, L.rank, L.ncand, st));
-    void* tmp = c.take<char>(scan_bytes);
-    Y5_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, L.flag, L.rank, L.ncand, st));
-    const long long threads = (long long)L.ncand * 32;
-    k_rows<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(L);
-    Y5_LAUNCH_CHECK();
-  } else {
-    // no targets: rank/flag single dummy entry = 0 so that level_rows() == 0
-    Y5_CUDA(cudaMemsetAsync(L.flag, 0, sizeof(int), st));
-    Y5_CUDA(cudaMemsetAsync(L.rank, 0, sizeof(int), st));
-  }
-  for (int lvl = 0; lvl < L.nl; ++lvl) {
-    k_obj<<<L.obj_blocks[lvl], OBJ_THREADS, 0, st>>>(L, lvl);
-    Y5_LAUNCH_CHECK();
-  }
-  if (L.ncand == 0) L.ncand = 1;  // k_final reads rank[ncand-1] + flag[ncand-1]
-  k_final<<<1, 256, 0, st>>>(L, loss1, items4);
-  Y5_LAUNCH_CHECK();
-  return Y5OBB_OK;
+  return forward(L, nullptr, loss1, items4, (cudaStream_t)stream);
+}
+
+size_t y5obb_loss_head_workspace_bytes(const y5obb_loss_desc* d, const y5obb_loss_head* head) {
+  y5obb_loss_desc dd;
+  HeadK hk;
+  LossK L;
+  size_t need = 0;
+  if (head_desc(d, head, &dd, &hk) != Y5OBB_OK || fill(L, &dd, nullptr, 0, &need, true) != Y5OBB_OK) return 0;
+  return need;
+}
+
+int y5obb_loss_forward_head(const y5obb_loss_desc* d, const y5obb_loss_head* head, float* loss1, float* items4,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  if (!loss1 || !items4 || !workspace) return Y5OBB_EINVAL;
+  y5obb_loss_desc dd;
+  HeadK hk;
+  int rc = head_desc(d, head, &dd, &hk);
+  if (rc) return rc;
+  LossK L;
+  size_t need = 0;
+  rc = fill(L, &dd, workspace, workspace_bytes, &need, true);
+  if (rc) return rc;
+  return forward(L, &hk, loss1, items4, (cudaStream_t)stream);
 }
 
 int y5obb_loss_backward(const y5obb_loss_desc* d, const float* grad_loss, void* workspace, size_t workspace_bytes,

@@ -284,18 +284,31 @@ class InferenceEngine:
                                    f"tensor on {device}, got {tuple(det_out.shape)} {det_out.dtype}")
             self.pred = det_out
         row_off = int(det_row_base)
+        # what ComputeLoss.head_items needs to check the Detect it is given and to recompute the head's logits
+        self.det_nl = det.nl
+        self.det_anchors = [float(v) for v in det.anchors.detach().float().cpu().flatten().tolist()]
+        self.det_strides = [float(s) for s in det.stride]
+        self._head = []
         for l, f in ((l, det.f[l]) for l in self.levels):
             cur[0] = ("Detect", l)
             mi = det.m[l]
             stride = float(det.stride[l])
             anchors_px = (det.anchors[l].detach().float().cpu() * stride).flatten().tolist()
-            add_conv(out[f], mi.weight.detach().float().cpu(), mi.bias.detach().float().cpu(), 1, 1, 0, False,
+            w, b = mi.weight.detach().float().cpu(), mi.bias.detach().float().cpu()
+            add_conv(out[f], w, b, 1, 1, 0, False,
                      detd=dict(out=self.pred, rows_per_image=self.pred.shape[1], row_off=row_off, no=det.no,
                                decode=2 if compact_detect else True,
                                stride=stride, anchors_px=anchors_px, descale=descale))
+            # the GEMM's operands: pack_weights rounds the same fp32 values to bf16, the bias stays fp32
+            self._head.append((out[f], w.reshape(w.shape[0], -1).to(torch.bfloat16).to(device), b.to(device)))
             row_off += det.na * hw[f][0] * hw[f][1]
         self.hbm_bytes += 4.0 * B * self.rows_total * det.no + 4.0 * B * 3 * H * W + 2.0 * self.x_s2d.numel()
         self.n_launches = len(self.ops) + 1
+
+    def head_inputs(self):
+        """Per emitted Detect level: (input Slice, bf16 weight [na * no, C], fp32 bias [na * no]) - the Detect GEMM's operands.
+        The input holds the features of the last forward until the next one, as `pred` does."""
+        return list(self._head)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         """x: [B,3,H,W] fp32 in [0,1] (or uint8 0..255) on this engine's device -> pred [B, A, no] fp32

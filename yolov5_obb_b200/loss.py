@@ -8,7 +8,7 @@ Focal loss (fl_gamma > 0) is outside the hot path (every shipped hyp sets 0,
 data/hyps/obb/hyp.finetune_dota.yaml:19) and is refused loudly.
 """
 import ctypes
-from ctypes import c_void_p, c_int, c_float
+from ctypes import c_void_p, c_int, c_int64, c_float
 
 import torch
 
@@ -25,6 +25,14 @@ class LossDesc(ctypes.Structure):
         ("anchor_t", c_float), ("cp", c_float), ("cn", c_float),
         ("hyp_box", c_float), ("hyp_obj", c_float), ("hyp_cls", c_float), ("hyp_theta", c_float),
         ("cls_pw", c_float), ("obj_pw", c_float), ("theta_pw", c_float), ("csl_sigma", c_float),
+    ]
+
+
+class LossHead(ctypes.Structure):
+    """Mirror of y5obb_loss_head (include/y5obb.h)."""
+    _fields_ = [
+        ("feat", c_void_p * 3), ("pix_stride", c_int64 * 3), ("row_stride", c_int64 * 3), ("img_stride", c_int64 * 3),
+        ("H", c_int * 3), ("W", c_int * 3), ("C", c_int * 3), ("w", c_void_p * 3), ("bias", c_void_p * 3),
     ]
 
 
@@ -93,20 +101,26 @@ class ComputeLoss:
         self._stride_host = [float(s) for s in self.stride]
 
     def _desc(self, ps, tg, grads=None) -> LossDesc:
-        d = LossDesc()
         no = ps[0].shape[-1]
+        d = self._base_desc(ps[0].shape[0], no, tg)
         for i, x in enumerate(ps):
             if x.dtype != torch.float32 or x.dim() != 5 or x.shape[-1] != no:
                 raise RuntimeError("predictions must be fp32 [B, na, H, W, no] tensors")
             d.p[i] = x.data_ptr()
             d.H[i], d.W[i] = x.shape[2], x.shape[3]
-            d.stride[i] = self._stride_host[i]
-            d.balance[i] = self.balance[i]
             if grads is not None:
                 d.grad[i] = grads[i].data_ptr()
+        return d
+
+    def _base_desc(self, B, no, tg) -> LossDesc:
+        """Everything but the logits and their shapes."""
+        d = LossDesc()
+        for i in range(self.nl):
+            d.stride[i] = self._stride_host[i]
+            d.balance[i] = self.balance[i]
         for i, v in enumerate(self._anchors_host):
             d.anchors[i] = v
-        d.nl, d.B, d.na, d.no, d.nc = self.nl, ps[0].shape[0], self.na, no, self.nc
+        d.nl, d.B, d.na, d.no, d.nc = self.nl, B, self.na, no, self.nc
         d.targets, d.nt, d.tcols = (tg.data_ptr() if tg.numel() else None), tg.shape[0], tg.shape[1] if tg.dim() == 2 else 187
         h = self.hyp
         d.anchor_t, d.cp, d.cn = h["anchor_t"], self.cp, self.cn
@@ -132,6 +146,47 @@ class ComputeLoss:
         _lib.require_cuda(targets, "targets")
         ps = [x.float() for x in p]  # AMP half predictions are widened; autograd casts the gradient back
         return _LossFn.apply(self, targets, *ps)
+
+
+    def head_items(self, engine, targets):
+        """val.py:198-199's `compute_loss([x.float() for x in train_out], targets)[1]` for the eval forward an
+        engine.InferenceEngine (Model.records_plan) has just run, without its raw head output: the loss reads logits computed
+        from the Detect inputs the plan keeps (y5obb_loss_forward_head).  targets: CUDA [nt, 187 | 8 | 7] as in __call__.
+        Returns device (loss [1], items [4]) = (lbox, lobj, lcls, ltheta); asynchronous, no autograd.  The features must still
+        be those of the batch the targets belong to: call it before the plan's next forward."""
+        from .engine import InferenceEngine
+        if not isinstance(engine, InferenceEngine):
+            raise RuntimeError(f"head_items needs an engine.InferenceEngine (one scale, every Detect level), got "
+                               f"{type(engine).__name__}")
+        if engine.levels != tuple(range(self.nl)):
+            raise RuntimeError(f"the plan emits Detect levels {engine.levels}; the loss needs all {self.nl}")
+        if (engine.det_nl, engine.na, engine.nc, engine.det_anchors, engine.det_strides) != (
+                self.nl, self.na, self.nc, self._anchors_host, self._stride_host):
+            raise RuntimeError("the plan's Detect (nl, na, nc, anchors, strides) differs from the one this loss was built for")
+        _lib.require_cuda(targets, "targets")
+        dev = engine.device
+        if targets.device != dev:
+            raise RuntimeError(f"targets are on {targets.device}, the plan on {dev}")
+        tg = targets.detach().float().contiguous()
+        d = self._base_desc(engine.B, engine.no, tg)
+        h = LossHead()
+        for i, (x, w, b) in enumerate(engine.head_inputs()):
+            h.feat[i] = x.ptr
+            h.pix_stride[i], h.row_stride[i], h.img_stride[i] = x.pix_stride, x.W * x.pix_stride, x.H * x.W * x.pix_stride
+            h.H[i], h.W[i], h.C[i] = x.H, x.W, x.C
+            h.w[i], h.bias[i] = w.data_ptr(), b.data_ptr()
+        L = _lib.lib()
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        items = torch.empty(4, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            nbytes = L.y5obb_loss_head_workspace_bytes(ctypes.byref(d), ctypes.byref(h))
+            if nbytes == 0:
+                raise RuntimeError("y5obb_loss_head_workspace_bytes: invalid loss description or Detect inputs")
+            st = _lib.stream_ptr(dev)
+            ws = _lib.workspace(nbytes, dev, f"loss_head:{st}")
+            _lib.check(L.y5obb_loss_forward_head(ctypes.byref(d), ctypes.byref(h), loss.data_ptr(), items.data_ptr(),
+                                                 ws.data_ptr(), ws.numel(), st), "y5obb_loss_forward_head")
+        return loss, items
 
 
 def compact_csl_index(theta_rad, num_class: int = 180):

@@ -223,15 +223,25 @@ class Validator:
     cls, cx, cy, l, s, theta, ...) in network-input pixels, shapes per image ((h_raw, w_raw), ((gain, gain), (pad_x, pad_y))).
     Per batch: upload, detect_records, non_max_suppression_obb(return_packed="async"), match_batch, ValStats.add - no host
     read.  A batch whose NMS candidates overflowed the optimistic capacity is not appended; its skip flag is read one batch
-    late, while the next batch computes, and the batch is then re-run with the blocking NMS from its device copy."""
+    late, while the next batch computes, and the batch is then re-run with the blocking NMS from its device copy.
+    compute_loss (a loss.ComputeLoss, train.py:364-373): the validation loss of val.py:198-199 is added per batch from the
+    plan's Detect inputs (ComputeLoss.head_items) into a device fp32 sum, and `results` becomes val.py:333's
+    (mp, mr, map50, map, box, obj, cls, theta) with the loss sum divided by the number of batches."""
 
     def __init__(self, model, conf_thres: float = 0.01, iou_thres: float = 0.4, max_det: int = 1500, iouv=None,
-                 augment: bool = False):
+                 augment: bool = False, compute_loss=None):
         self.model = model
         self.augment = bool(augment)   # val.py --augment: test-time augmentation (Model.detect_records(augment=True))
         self.device = _resolve(next(model.parameters()).device)
         if self.device.type != "cuda":
             raise RuntimeError("Validator needs the model on a CUDA device; there is no CPU path")
+        if compute_loss is not None and not hasattr(compute_loss, "head_items"):
+            raise RuntimeError("compute_loss must be a yolov5_obb_b200.loss.ComputeLoss (the loss is computed from the eval "
+                               "plan's Detect inputs)")
+        if compute_loss is not None and self.augment:
+            # the reference has no training outputs under augmentation either (train_out = None, val.py:199)
+            raise RuntimeError("the validation loss is not defined with test-time augmentation")
+        self.compute_loss = compute_loss
         self.nms = dict(conf_thres=conf_thres, iou_thres=iou_thres, multi_label=True, max_det=max_det)
         iouv = torch.linspace(0.5, 0.95, 10) if iouv is None else iouv
         self.iouv = iouv.detach().float().to(self.device)
@@ -240,22 +250,29 @@ class Validator:
     def __call__(self, batches) -> ValMetrics:
         stats = ValStats(self.model.model[-1].nc, self.iouv.numel(), self.device)
         pending = None
+        self._loss, n_batches = torch.zeros(4, dtype=torch.float32, device=self.device), 0
         with torch.cuda.device(self.device):
             for im, targets, _paths, shapes in batches:
                 cur = self._submit(stats, im, targets, shapes)
+                n_batches += 1
                 if pending is not None:
                     self._settle(stats, pending)
                 pending = cur
             if pending is not None:
                 self._settle(stats, pending)
-            return stats.metrics()
+            m = stats.metrics()
+        if self.compute_loss is not None:
+            m.results = m.results + tuple((self._loss.cpu() / n_batches).tolist())   # val.py:333
+        return m
 
     def _submit(self, stats, im, targets, shapes):
         from .general import non_max_suppression_obb
         x, t = _upload(im, self.device), _upload(targets.float(), self.device)
         base = stats.seen
-        dets, counts, cap = non_max_suppression_obb(self.model.detect_records(x, augment=self.augment), return_packed="async",
-                                                    **self.nms)
+        recs = self.model.detect_records(x, augment=self.augment)
+        if self.compute_loss is not None:   # val.py:198-199; the overflow re-run in _settle does not add it again
+            self._loss += self.compute_loss.head_items(self.model.records_plan(tuple(x.shape), x.device), t)[1]
+        dets, counts, cap = non_max_suppression_obb(recs, return_packed="async", **self.nms)
         correct, _, _ = match_batch(dets, counts, t, shapes, self.iouv, want_geometry=False)
         skip = stats.add(dets, counts, correct, t, nms_cap=cap)
         host = torch.empty(1, dtype=torch.int32).pin_memory()
