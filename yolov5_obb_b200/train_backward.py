@@ -18,6 +18,7 @@ import torch
 
 from . import _lib
 from .conv import Conv as ConvOp, Slice, pack_weights, tiling, MODE_DETECT
+from .train_engine import flat_layout
 from .train_ops import Wgrad
 
 
@@ -82,30 +83,39 @@ class BackwardPlan:
         written = _Written()
         det = eng.model.model[-1]
 
+        # activation-sized buffers come from the engine's allocator (its arena when one is reserved, train_engine.TrainArena);
+        # `zero=True` marks the ones a launch relies on being zero where nothing writes them
+        carve = eng._carver.take
+
         def gslice(s: Slice) -> Slice:
             k = s.buf.data_ptr()
             if k not in self.gbuf:
-                self.gbuf[k] = torch.zeros_like(s.buf)
+                self.gbuf[k] = carve(tuple(s.buf.shape), s.buf.dtype)
             return Slice(self.gbuf[k], s.c_off, s.C)
 
         def f32(n):
-            t = torch.zeros(n, dtype=torch.float32, device=dev)
+            t = carve((n,), torch.float32)
             self.keep.append(t)
             return t
 
-        def bf(*shape):
-            t = torch.zeros(shape, dtype=torch.bfloat16, device=dev)
+        def bf(*shape, zero=False):
+            t = carve(shape, torch.bfloat16, zero=zero)
             self.keep.append(t)
             return t
 
         # one flat fp32 buffer holds every parameter gradient (model.parameters() order): the kernels write into
         # views of it, a data-parallel job all-reduces it in one call
+        # (with an arena, the arena's: every training shape writes the same buffer, so the fused optimizer step's table and
+        # a data-parallel all-reduce see one buffer whatever the shape)
         self.params = [p for p in eng.model.parameters()]
-        self.offsets, n = [], 0
-        for p in self.params:
-            self.offsets.append(n)
-            n += (p.numel() + 3) // 4 * 4  # 16-byte aligned views
-        self.flat = torch.zeros(n, dtype=torch.float32, device=dev)
+        self.offsets, n = flat_layout(self.params)
+        self.arena = eng.arena
+        if self.arena is not None:
+            if self.arena.flat.numel() != n:
+                raise RuntimeError("the training arena was reserved for a different set of parameters")
+            self.flat = self.arena.flat
+        else:
+            self.flat = torch.zeros(n, dtype=torch.float32, device=dev)
         self.pgrad: Dict[torch.nn.Parameter, torch.Tensor] = {
             p: self.flat[o:o + p.numel()].view(p.shape) for p, o in zip(self.params, self.offsets)}
 
@@ -124,7 +134,7 @@ class BackwardPlan:
             return op, wp
 
         # ---------------- Detect levels ----------------
-        self.det_grads_in = [torch.zeros_like(o) for o in eng.det_out]  # static copies of dLoss/dpred (graph inputs)
+        self.det_grads_in = [carve(tuple(o.shape), o.dtype) for o in eng.det_out]  # static copies of dLoss/dpred (graph inputs)
         self._calls, self._graph = 0, None
         self.det_parts = []
         for l in range(det.nl):
@@ -278,7 +288,7 @@ class BackwardPlan:
                             part["dgrad_ops"].append(op)
                             self.keep.append(op)
                 else:
-                    dzup = bf(B, x.H, x.W, Cout)
+                    dzup = bf(B, x.H, x.W, Cout, zero=True)   # odd positions: zero, never written by zero_stuff2x
                     add("zero_stuff", lambda st, dz=dz, dzup=dzup, npix=npix, C=Cout, W=Ww:
                                       _lib.check(L.y5obb_zero_stuff2x(dz.data_ptr(), C, dzup.data_ptr(), C, npix, C, W, st), "zero_stuff"))
                     op, wp = add_dgrad(Slice.full(dzup), w_d, k, k - 1 - p, gx, "dgrad s2")
@@ -325,11 +335,13 @@ class BackwardPlan:
                     self._launch_all(st)
                 else:
                     if self._graph is None:
+                        mem0 = torch.cuda.memory_allocated(eng.device)
                         torch.cuda.synchronize(eng.device)
                         g = torch.cuda.CUDAGraph()
                         with torch.cuda.graph(g, capture_error_mode="thread_local"):
                             self._launch_all(_lib.stream_ptr(eng.device))
                         self._graph = g
+                        eng.outside_bytes += torch.cuda.memory_allocated(eng.device) - mem0
                     self._graph.replay()
         return self.flat
 

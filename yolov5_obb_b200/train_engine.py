@@ -6,6 +6,7 @@ kept for the backward pass.  Mirrors models/yolo.py:163-181 (_forward_once) in t
 Differences from the inference plan (engine.py): BN is not folded, nothing is updated in place (backward needs
 every activation), cv1/cv2 of a C3 run as separate GEMMs (each has its own BatchNorm), and the raw conv output z
 of every layer is stored next to its activated output y."""
+import weakref
 from typing import Dict, List, Optional
 
 import torch
@@ -13,6 +14,79 @@ import torch
 from . import _lib
 from .conv import Conv as ConvOp, Slice, WindowView, pack_weights, MODE_DETECT
 from .engine import _is
+
+
+def flat_layout(params):
+    """Offsets of every parameter's gradient in the flat fp32 buffer (16-byte aligned views) and its length."""
+    offsets, n = [], 0
+    for p in params:
+        offsets.append(n)
+        n += (p.numel() + 3) // 4 * 4
+    return offsets, n
+
+
+class TrainArena:
+    """One device allocation that every training plan of a model carves its activation, raw-output, Detect-logit and
+    gradient buffers from (Model.reserve_train_arena), plus the one flat parameter-gradient buffer all plans share.
+
+    Plans of different shapes alias the same bytes: only one plan runs at a time, on one stream (the backward's wgrad
+    stream joins it before the backward returns).  `owner` is the plan whose data the arena holds; a plan that runs after
+    another one re-zeroes the few regions it relies on being zero (TrainEngine.zero_regions) before its first launch."""
+
+    ALIGN = 256
+
+    def __init__(self, nbytes: int, n_flat: int, device):
+        self.device = torch.device(device)
+        self.buf = torch.empty(int(nbytes), dtype=torch.uint8, device=self.device)
+        self.flat = torch.zeros(n_flat, dtype=torch.float32, device=self.device)
+        self.owner = None   # weak reference to the TrainEngine whose data the arena holds
+        self.last_grad_flat = None   # the clone of the flat gradient the last backward handed to autograd
+        self._inputs = {}
+
+    @property
+    def nbytes(self) -> int:
+        return self.buf.numel()
+
+    def input_buffer(self, shape, dtype) -> torch.Tensor:
+        """The static input of the captured forward graphs, one per (shape, dtype) for all plans."""
+        key = (tuple(shape), dtype)
+        t = self._inputs.get(key)
+        if t is None:
+            t = self._inputs[key] = torch.empty(key[0], dtype=dtype, device=self.device)
+        return t
+
+
+class _Carver:
+    """Bump allocator over a TrainArena (arena=None: ordinary zero-filled allocations whose arena offsets are still
+    counted, which is how Model.reserve_train_arena sizes the arena)."""
+
+    def __init__(self, arena: Optional[TrainArena], device):
+        self.arena, self.device, self.off = arena, device, 0
+        self.zero = []   # regions the plan relies on being zero
+
+    def take(self, shape, dtype, zero: bool = False) -> torch.Tensor:
+        n = 1
+        for s in shape:
+            n *= int(s)
+        nbytes = n * torch.empty((), dtype=dtype).element_size()
+        a = TrainArena.ALIGN
+        off = (self.off + a - 1) // a * a
+        self.off = off + nbytes
+        if self.arena is None:
+            return torch.zeros(tuple(shape), dtype=dtype, device=self.device)
+        if self.off > self.arena.nbytes:
+            raise RuntimeError(f"training plan needs more than the {self.arena.nbytes} bytes of the reserved arena: "
+                               "reserve it for the largest batch and image size (Model.reserve_train_arena)")
+        t = self.arena.buf[off:off + nbytes].view(dtype).view(tuple(shape))
+        if zero:
+            self.zeroed(t)
+        return t
+
+    def zeroed(self, t: torch.Tensor):
+        """Register a view of an arena buffer that must read as zero whenever the plan runs (and zero it now)."""
+        if self.arena is not None:
+            t.zero_()
+            self.zero.append(t)
 
 
 class _BNLayer:
@@ -33,7 +107,12 @@ class _BNLayer:
 
 
 class TrainEngine:
-    def __init__(self, model, B: int, H: int, W: int, device):
+    def __init__(self, model, B: int, H: int, W: int, device, in_hw=None, arena: Optional[TrainArena] = None,
+                 carver: Optional[_Carver] = None):
+        """in_hw: (H_in, W_in) of the input when it differs from the planned (H, W): the plan's first launch is then the
+        bilinear resize of train.py's --multi-scale (F.interpolate, align_corners=False) straight into the stem input.
+        arena: carve every activation / gradient buffer from that TrainArena (Model.reserve_train_arena); carver: an
+        explicit allocator (the arena sizing pass)."""
         device = torch.device(device)
         if device.type != "cuda":
             raise RuntimeError("TrainEngine needs a CUDA device (sm_90a); there is no CPU path")
@@ -42,6 +121,10 @@ class TrainEngine:
         if H % smax or W % smax:
             raise RuntimeError(f"image size {H}x{W} must be a multiple of the max stride {smax}")
         self.device, self.B, self.H, self.W = device, B, H, W
+        self.in_hw = (H, W) if in_hw is None else (int(in_hw[0]), int(in_hw[1]))
+        self.arena = arena
+        self._carver = carver if carver is not None else _Carver(arena, device)
+        mem0 = torch.cuda.memory_allocated(device)
         self.model = model
         self.layers: List[_BNLayer] = []
         self.pre_ops, self.keep = [], []
@@ -74,7 +157,7 @@ class TrainEngine:
                 ch[i], hw[i] = sum(ch[f] for f in fs), in_hw
 
         def new(h, w, c):
-            t = torch.zeros((B, h, w, c), dtype=torch.bfloat16, device=device)
+            t = self._carver.take((B, h, w, c), torch.bfloat16)
             self.keep.append(t)
             return t
 
@@ -131,7 +214,9 @@ class TrainEngine:
             self.layers.append(lay)
             return lay
 
-        self.x_s2d = torch.zeros((B, H // 2, W // 2 + 2, 16), dtype=torch.bfloat16, device=device)
+        self.x_s2d = self._carver.take((B, H // 2, W // 2 + 2, 16), torch.bfloat16)
+        self._carver.zeroed(self.x_s2d[:, :, 0])    # the pad columns: the stem kernels never write them
+        self._carver.zeroed(self.x_s2d[:, :, -1])
         self.sppf = None
         for m in mods:
             i = m.i
@@ -176,7 +261,10 @@ class TrainEngine:
         for l, f in enumerate(det.f):
             mi = det.m[l]
             hh, ww = hw[f]
-            o = torch.empty((B, det.na, hh, ww, det.no), dtype=torch.float32, device=device)
+            if arena is None and carver is None:
+                o = torch.empty((B, det.na, hh, ww, det.no), dtype=torch.float32, device=device)
+            else:
+                o = self._carver.take((B, det.na, hh, ww, det.no), torch.float32)
             wp, bp = pack_weights(mi.weight.detach().float(), mi.bias.detach().float(), MODE_DETECT, det.no)
             stride = float(det.stride[l])
             cv = ConvOp(out[f], wp, bp, mi.weight.shape[0], 1, 1, 0, False,
@@ -194,6 +282,21 @@ class TrainEngine:
         self._nbt = [lay.mod.bn.num_batches_tracked for lay in self.layers if not isinstance(lay, tuple)]
         cmax = max([lay.z.C for lay in self.layers if not isinstance(lay, tuple)] + [det.na * 256])
         self.scratch = torch.zeros(int(L.y5obb_bn_scratch_floats(cmax)), dtype=torch.float32, device=device)  # reductions
+        # device bytes this plan holds outside the arena (BatchNorm vectors, packed weights, scratch; later the backward
+        # plan's and the captured graphs'): with an arena, what each additional training shape costs
+        self.outside_bytes = torch.cuda.memory_allocated(device) - mem0
+
+    @property
+    def zero_regions(self) -> List[torch.Tensor]:
+        """Arena views this plan (forward and backward) relies on being zero: re-zeroed when it runs after another plan."""
+        return list(self._carver.zero)
+
+    def _claim_arena(self):
+        a = self.arena
+        if a is not None and (a.owner is None or a.owner() is not self):
+            for t in self._carver.zero:
+                t.zero_()
+            a.owner = weakref.ref(self)
 
     @staticmethod
     def _stem_weight(w):
@@ -231,10 +334,11 @@ class TrainEngine:
         The launch sequence is fixed (same buffers every step), so from the third call on it is replayed as ONE CUDA
         graph per input dtype: ~330 launches collapse into a single cudaGraphLaunch (Y5OBB_NO_GRAPH=1 disables)."""
         _lib.require_cuda(x, "x")
-        if tuple(x.shape) != (self.B, 3, self.H, self.W):
-            raise RuntimeError(f"engine was planned for {(self.B, 3, self.H, self.W)}, got {tuple(x.shape)}")
+        if tuple(x.shape) != (self.B, 3) + self.in_hw:
+            raise RuntimeError(f"engine was planned for {(self.B, 3) + self.in_hw}, got {tuple(x.shape)}")
         if x.dtype != torch.uint8:
             x = x.float()
+        self._claim_arena()
         if self.prof is not None or not self.use_graph:
             return self._forward_eager(x.contiguous(), refresh)
         slot = self._graphs.setdefault((x.dtype, refresh), dict(calls=0, graph=None, x=None))
@@ -244,13 +348,18 @@ class TrainEngine:
         if slot["graph"] is None:
             if refresh and self._pack is None:
                 self.refresh_weights()  # builds the packing plan (allocates): not capturable
-            slot["x"] = torch.empty_like(x, memory_format=torch.contiguous_format)
+            mem0 = torch.cuda.memory_allocated(self.device)
+            if self.arena is not None:   # one static input per shape for all plans of the arena
+                slot["x"] = self.arena.input_buffer(x.shape, x.dtype)
+            else:
+                slot["x"] = torch.empty_like(x, memory_format=torch.contiguous_format)
             slot["x"].copy_(x)
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, capture_error_mode="thread_local"):
                 self._forward_eager(slot["x"], refresh)
             slot["graph"] = g
+            self.outside_bytes += torch.cuda.memory_allocated(self.device) - mem0
         slot["x"].copy_(x)
         slot["graph"].replay()
         return self.det_out
@@ -272,7 +381,12 @@ class TrainEngine:
             evs.append((tag, e0, e1))
 
         with torch.cuda.device(self.device):
-            if x.dtype == torch.uint8:
+            if self.in_hw != (self.H, self.W):   # --multi-scale: bilinear resize (no flip, no pad) into the stem input
+                fn = L.y5obb_scale_img_s2d_u8 if x.dtype == torch.uint8 else L.y5obb_scale_img_s2d
+                Hi, Wi = self.in_hw
+                run("resize", lambda: fn(x.data_ptr(), self.x_s2d.data_ptr(), self.B, Hi, Wi, self.H, self.W, self.H, self.W,
+                                         0, 0.0, 1, st))
+            elif x.dtype == torch.uint8:
                 run("s2d", lambda: L.y5obb_stem_s2d_u8(x.data_ptr(), self.x_s2d.data_ptr(), self.B, self.H, self.W, 1, st))
             else:
                 run("s2d", lambda: L.y5obb_stem_s2d(x.data_ptr(), self.x_s2d.data_ptr(), self.B, self.H, self.W, 1, st))
@@ -308,7 +422,9 @@ class TrainEngine:
         gradient (fp32, model.parameters() order, see train_backward.py)."""
         if self._bwd is None:
             from .train_backward import BackwardPlan
+            mem0 = torch.cuda.memory_allocated(self.device)
             self._bwd = BackwardPlan(self)     # packs its data-gradient weights from the current parameters
+            self.outside_bytes += torch.cuda.memory_allocated(self.device) - mem0
             self._pack = None                  # the next refresh_weights() covers them too ...
             self._graphs = {}                  # ... so captured forward graphs (old packing plan) are dropped
         self._bwd.run(grads)

@@ -11,6 +11,7 @@ SGD with Nesterov momentum (train.py:158), ModelEMA as utils/torch_utils.py:284-
 The device computes in bf16 with fp32 accumulation and fp32 master weights: no loss scaling is needed (the reference's
 GradScaler exists for fp16 autocast, train.py:246,333-337)."""
 import math
+import random
 from copy import deepcopy
 from typing import Optional
 
@@ -37,6 +38,30 @@ def param_groups(model):
         elif hasattr(v, "weight") and isinstance(v.weight, nn.Parameter):
             g1.append(v.weight)
     return g0, g1, g2
+
+
+def multi_scale_shape(imgsz: int, gs: int, H: int, W: int, rng: random.Random):
+    """train.py:314-318 (--multi-scale) for a batch of H x W images: one draw from `rng` -> (ns_h, ns_w, label_ratio).
+    The reference passes float bounds to randrange, which Python 3.12 refuses; their integral values give the draws Python
+    3.8-3.11 gave."""
+    sz = rng.randrange(int(imgsz * 0.5), int(imgsz * 1.5 + gs)) // gs * gs
+    return _scaled_shape(sz, gs, H, W)
+
+
+def _scaled_shape(sz: int, gs: int, H: int, W: int):
+    """sf == 1 leaves the batch alone: (H, W, 1.0).  The fp64 ceil is kept as written: for some sizes it rounds up one grid
+    step (imgsz 800, sz 448 -> 480)."""
+    sf = sz / max(H, W)
+    if sf == 1:
+        return H, W, 1.0
+    ns = [math.ceil(x * sf / gs) * gs for x in (H, W)]
+    return ns[0], ns[1], float(ns[0]) / H
+
+
+def multi_scale_max_shape(imgsz: int, gs: int, H: int, W: int):
+    """The largest (ns_h, ns_w) multi_scale_shape can return for H x W batches."""
+    shapes = [_scaled_shape(v // gs * gs, gs, H, W) for v in range(int(imgsz * 0.5), int(imgsz * 1.5 + gs))]
+    return max(s[0] for s in shapes), max(s[1] for s in shapes)
 
 
 class ModelEMA:
@@ -76,10 +101,19 @@ class TrainStep:
     """model: yolov5_obb_b200.yolo.Model on a CUDA device, in train() mode.  step(imgs, targets) -> (loss, loss_items)."""
 
     def __init__(self, model, hyp: Optional[dict] = None, batch_size: int = 16, imgsz: int = 1024, ema: bool = True,
-                 warmup_iters: int = 0):
+                 warmup_iters: int = 0, multi_scale: bool = False, seed: Optional[int] = None):
         """warmup_iters > 0: the warm-up of train.py:305-316 over that many iterations (the reference uses
         max(round(warmup_epochs * batches_per_epoch), 1000)): every group's lr is interpolated from 0 (biases: from
-        hyp['warmup_bias_lr']) to lr0 and the momentum from hyp['warmup_momentum'] to hyp['momentum']."""
+        hyp['warmup_bias_lr']) to lr0 and the momentum from hyp['warmup_momentum'] to hyp['momentum'].
+
+        multi_scale=True: train.py --multi-scale (train.py:312-320).  Every step draws a size (multi_scale_shape), resizes
+        the batch on the device as the plan's first launch and scales targets[:, 2:6] into a buffer the step owns (the
+        caller's targets are left as they are; the reference scales them in place).  The draws come from a
+        random.Random(seed) owned by the step, seed=None meaning train.py's init_seeds(1 + RANK): the module-level
+        `random` stays the augmentation's (augment.DeviceAugmentLoader), as in the reference with dataloader workers,
+        where the main process draws nothing else from it.  The constructor reserves one training arena
+        (Model.reserve_train_arena) for batch_size images of the largest drawable size, assuming imgsz x imgsz batches
+        (no --rect), so an out-of-memory error shows at start-up.  `last_shape` is the (h, w) the last step trained at."""
         self.model = model
         self.hyp = dict(HYP_FINETUNE_DOTA if hyp is None else hyp)
         nbs = 64
@@ -94,6 +128,12 @@ class TrainStep:
         model.hyp = self.hyp
         model.nc = model.model[-1].nc
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        rank = dist.get_rank() if self.world > 1 else -1
+        self.multi_scale, self.imgsz = bool(multi_scale), int(imgsz)
+        self.gs = max(int(model.stride.max()), 32)                     # train.py:134
+        self.rng = random.Random(1 + rank if seed is None else seed)
+        self.last_shape = None
+        self._tg = None
         if self.world > 1:
             # DDP broadcasts rank 0's parameters and buffers when it wraps the model (train.py:214); the reference seeds
             # per rank (train.py:100), so without this the replicas would start from different weights.  Done BEFORE the
@@ -119,6 +159,9 @@ class TrainStep:
         self._fused = None
         self._use_fused = (self.accumulate == 1 and os.environ.get("Y5OBB_FUSED_SGD", "1") != "0"
                            and next(model.parameters()).is_cuda and hasattr(model, "_bump_generation"))
+        if self.multi_scale:
+            hmax, wmax = multi_scale_max_shape(self.imgsz, self.gs, self.imgsz, self.imgsz)
+            model.reserve_train_arena(batch_size, hmax, wmax, next(model.parameters()).device)
 
     def step(self, imgs: torch.Tensor, targets: torch.Tensor):
         """imgs: uint8 or float [B,3,H,W] on the device; targets [nt, 187] (image index, class, cx, cy, l, s, theta, CSL row)."""
@@ -130,7 +173,18 @@ class TrainStep:
                 g["lr"] = lo + f * (self.hyp["lr0"] - lo)
                 if "momentum" in g:
                     g["momentum"] = self.hyp["warmup_momentum"] + f * (self.hyp["momentum"] - self.hyp["warmup_momentum"])
-        pred = model(imgs)                                  # uint8 is normalised inside the stem's loader kernel
+        size = None
+        if self.multi_scale:                                # train.py:312-320
+            H, W = int(imgs.shape[2]), int(imgs.shape[3])
+            nh, nw, ratio = multi_scale_shape(self.imgsz, self.gs, H, W, self.rng)
+            if (nh, nw) != (H, W):
+                size = (nh, nw)
+                targets = self._scale_targets(targets, ratio)
+            self.last_shape = (nh, nw)
+            pred = model.forward_train(imgs, size)          # the resize is the plan's first launch
+        else:
+            self.last_shape = (int(imgs.shape[2]), int(imgs.shape[3]))
+            pred = model(imgs)                              # uint8 is normalised inside the stem's loader kernel
         loss, items = self.compute_loss(pred, targets)
         loss.backward()                                     # (x WORLD_SIZE of train.py:328 is folded into the SUM below)
         if self.ni - self._last_opt >= self.accumulate:
@@ -146,6 +200,20 @@ class TrainStep:
             self._last_opt = self.ni
         self.ni += 1
         return loss.detach(), items
+
+    def _scale_targets(self, targets: torch.Tensor, ratio: float) -> torch.Tensor:
+        """targets[:, 2:6] * label_ratio (cx, cy, l, s in the 187-, 8- and 7-column layouts; fp32 as ATen's in-place
+        multiply computes it) in a buffer the step owns, reused (stream-ordered) by later steps."""
+        nt = int(targets.shape[0])
+        t = self._tg
+        if t is None or t.shape[0] < nt or t.shape[1:] != targets.shape[1:] or t.dtype != targets.dtype or \
+                t.device != targets.device:
+            t = self._tg = torch.empty((max(nt, 64) * 2,) + tuple(targets.shape[1:]), dtype=targets.dtype,
+                                       device=targets.device)
+        out = t[:nt]
+        out.copy_(targets)
+        out[:, 2:6].mul_(ratio)
+        return out
 
     def run(self, host_batches):
         """The batch loop of train.py:296-342 over HOST batches (what the dataloader yields: pinned uint8 images [B,3,H,W] and
@@ -235,12 +303,13 @@ class TrainStep:
         plan = model._last_train_engine._bwd
         if self.world > 1:
             dist.all_reduce(plan.flat, op=dist.ReduceOp.SUM)
-        if self._fused is None or self._fused_plan is not plan:
+        key = plan.flat if plan.arena is not None else plan   # (an arena's flat buffer is shared by every shape)
+        if self._fused is None or self._fused_plan is not key:
             groups = [g["params"] for g in self.optimizer.param_groups]
             self._fused = FusedSGDEMA(model, groups, plan.pgrad, self.ema.ema if self.ema is not None else None,
                                       weight_decay=self.hyp["weight_decay"], momentum_buffers=getattr(self, "_mom", None))
             self._mom = self._fused.mom
-            self._fused_plan = plan
+            self._fused_plan = key
             for p, m in self._fused.mom.items():
                 self.optimizer.state[p]["momentum_buffer"] = m
         g = self.optimizer.param_groups
@@ -261,6 +330,8 @@ class TrainStep:
         tensors) are reduced one by one."""
         params = [p for p in self.model.parameters() if p.grad is not None]
         eng = getattr(self.model, "_last_train_engine", None)
+        if getattr(eng, "arena", None) is not None:
+            eng = eng.arena
         cands = [getattr(eng, "last_grad_flat", None)]
         if params and params[0].grad._base is not None:   # gradient accumulation: .grad still views the FIRST step's buffer
             cands.append(params[0].grad._base)

@@ -7,6 +7,7 @@ reference state_dict loads unchanged), same forward() return values.  The module
 parameters; all arithmetic runs in csrc/ through the C ABI (engine.py).  There is no PyTorch compute
 path in this package — the fp32 torch restatement used by the tests lives in oracle/model_ref.py.
 """
+import gc
 import math
 from copy import deepcopy
 from pathlib import Path
@@ -183,7 +184,9 @@ class _TrainFn(torch.autograd.Function):
         # one clone of the flat buffer: autograd may keep the returned views as .grad (zero_grad(set_to_none=True) makes
         # that copy-free), and the plan rewrites its own buffer every step
         flat = plan.flat.clone()
-        ctx.eng.last_grad_flat = flat
+        # (one reference for all plans of an arena: a clone kept per shape would cost a flat buffer per shape)
+        arena = getattr(ctx.eng, "arena", None)
+        (arena if arena is not None else ctx.eng).last_grad_flat = flat
         views = {p: flat[o:o + p.numel()].view(p.shape) for p, o in zip(plan.params, plan.offsets)}
         return (None, None) + tuple(views.get(p) for p in ctx.params)
 
@@ -278,7 +281,7 @@ class Model(nn.Module):
         """copy.deepcopy(model) (ModelEMA, checkpoints): parameters and buffers are copied, the device plans are not."""
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
-        skip = ("_engines", "_last_train_engine", "_sig_tensors", "_sig_nbt")
+        skip = ("_engines", "_last_train_engine", "_sig_tensors", "_sig_nbt", "_train_arena")
         new.__dict__ = {k: deepcopy(v, memo) for k, v in self.__dict__.items() if k not in skip}
         new._engines = {}
         new._sig_tensors = None
@@ -294,19 +297,7 @@ class Model(nn.Module):
         if augment or profile or visualize:
             raise RuntimeError("augment/profile/visualize are host tooling outside the hot path")
         if self.training:
-            from .train_engine import TrainEngine
-            key = ("train", tuple(x.shape), x.device.index)
-            eng = self._engines.get(key)
-            refresh = eng is not None          # an existing plan re-packs the (possibly updated) parameters first
-            if eng is None:
-                eng = self._engines[key] = TrainEngine(self, x.shape[0], x.shape[2], x.shape[3], x.device)
-            eng._refresh_next = refresh
-            self._last_train_engine = eng
-            self._bump_generation()  # running statistics move (the captured graph bumps no version counter)
-            if not torch.is_grad_enabled():
-                return eng.forward(x, refresh)
-            params = [p for p in self.parameters() if p.requires_grad]
-            return list(_TrainFn.apply(eng, x, *params))
+            return self.forward_train(x)
         from .engine import InferenceEngine
         key = (tuple(x.shape), x.device.index)
         eng = self._engines.get(key)
@@ -318,6 +309,71 @@ class Model(nn.Module):
             eng = self._engines[key] = InferenceEngine(self, x.shape[0], x.shape[2], x.shape[3], x.device)
             eng._weights_sig = sig
         return eng.forward(x), None
+
+    def forward_train(self, x, size=None):
+        """Training-mode forward (what forward(x) runs in train()): list of 3 raw [B, 3, H_i, W_i, nc+185] logits.
+        size=(h, w): train.py's --multi-scale resize, `F.interpolate(x, size=size, mode='bilinear', align_corners=False)`,
+        runs as the plan's first launch (the plan takes the un-resized x; plans are keyed by input shape and size).
+        With a reserved arena (reserve_train_arena) the returned tensors live in it: the next training forward of ANY
+        shape overwrites them."""
+        from .train_engine import TrainEngine
+        in_hw = (int(x.shape[2]), int(x.shape[3]))
+        hw = in_hw if size is None else (int(size[0]), int(size[1]))
+        key = ("train", tuple(x.shape), x.device.index) + ((hw,) if hw != in_hw else ())
+        eng = self._engines.get(key)
+        refresh = eng is not None          # an existing plan re-packs the (possibly updated) parameters first
+        if eng is None:
+            arena = getattr(self, "_train_arena", None)
+            if arena is not None and arena.device != x.device:
+                arena = None
+            eng = self._engines[key] = TrainEngine(self, x.shape[0], hw[0], hw[1], x.device, in_hw=in_hw, arena=arena)
+        eng._refresh_next = refresh
+        self._last_train_engine = eng
+        self._bump_generation()  # running statistics move (the captured graph bumps no version counter)
+        if not torch.is_grad_enabled():
+            return eng.forward(x, refresh)
+        params = [p for p in self.parameters() if p.requires_grad]
+        return list(_TrainFn.apply(eng, x, *params))
+
+    def reserve_train_arena(self, B, H_max, W_max, device):
+        """Carve the activation, raw-output, Detect-logit and gradient buffers of every training plan on `device` from ONE
+        allocation sized for a [B, 3, H_max, W_max] plan (train_engine.TrainArena), and give all of them one flat gradient
+        buffer.  Any plan of batch <= B and size <= H_max x W_max then fits: a multi-scale run costs the largest shape's
+        buffers once, plus per shape only what the plan reports as `outside_bytes` (BatchNorm vectors, packed weights,
+        graphs).  Running out of memory happens here, at start-up.  Training plans built before the call keep their own
+        buffers; plans bound to an earlier arena are dropped.  Returns the arena."""
+        from .train_backward import BackwardPlan
+        from .train_engine import TrainArena, TrainEngine, _Carver, flat_layout
+        device = torch.device(device)
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        old = getattr(self, "_train_arena", None)
+        if old is not None:
+            for k in [k for k, e in self._engines.items() if getattr(e, "arena", None) is old]:
+                del self._engines[k]
+            self._train_arena = None
+            del old
+        # sizing pass: the largest plan built with ordinary allocations, counting the arena offsets it would take
+        carver = _Carver(None, device)
+        with torch.no_grad():
+            eng = TrainEngine(self, int(B), int(H_max), int(W_max), device, carver=carver)
+            BackwardPlan(eng)
+        nbytes = carver.off
+        del eng
+        gc.collect()              # (the plans' launch closures form reference cycles)
+        torch.cuda.synchronize(device)
+        torch.cuda.empty_cache()
+        _, n_flat = flat_layout(list(self.parameters()))
+        self._train_arena = TrainArena(nbytes, n_flat, device)
+        return self._train_arena
+
+    def release_train_arena(self):
+        """Drop the arena and the training plans carved from it."""
+        arena = getattr(self, "_train_arena", None)
+        if arena is not None:
+            for k in [k for k, e in self._engines.items() if getattr(e, "arena", None) is arena]:
+                del self._engines[k]
+            self._train_arena = None
 
     def forward_augment(self, x):
         """models/yolo.py:149-161 _forward_augment on the device (test-time augmentation, `val.py --augment`,
