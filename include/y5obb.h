@@ -377,6 +377,29 @@ int y5obb_sgd_ema_plan_run(const y5obb_sgd_plan_t* plan, const float* lr3, float
                            void* stream);
 void y5obb_sgd_ema_plan_destroy(y5obb_sgd_plan_t* plan);
 
+/* ---- fused Adam + EMA step ---------------------------------------------------------------------------------------------
+ * train.py --adam (train.py:157-163): torch.optim.Adam's multi-tensor step (coupled L2 weight decay, amsgrad off) and
+ * utils/torch_utils.py:304-314 over every tensor in one launch, each op rounded as ATen's foreach kernels round it.  group
+ * 0/1/2 index the per-step step-size table; group -1 = EMA only (floating-point buffers); ema may be NULL.
+ * run: step_size3[k] = -lr_k / (1 - beta1^t) and bc2_sqrt = (1 - beta2^t)^0.5, computed in double and rounded to float as
+ * torch does; beta1 / beta2 are the doubles of the parameter group (1 - beta1, beta2 and 1 - beta2 are formed in double
+ * and rounded to float here, as torch's scalar arguments are).  beta1 and beta2 must lie in [0, 1), bc2_sqrt be > 0. */
+typedef struct y5obb_adam_plan y5obb_adam_plan_t;
+typedef struct {
+  float* p;           /* parameter (fp32 master weight), updated in place */
+  const float* g;     /* gradient */
+  float* exp_avg;     /* first moment */
+  float* exp_avg_sq;  /* second moment */
+  float* ema;         /* EMA copy of p, or NULL */
+  int64_t n;
+  float weight_decay;
+  int group;
+} y5obb_adam_entry;
+int y5obb_adam_ema_plan_create(const y5obb_adam_entry* entries, int n, y5obb_adam_plan_t** out);
+int y5obb_adam_ema_plan_run(const y5obb_adam_plan_t* plan, const float* step_size3, double beta1, double beta2,
+                            float bc2_sqrt, float eps, float ema_decay, void* stream);
+void y5obb_adam_ema_plan_destroy(y5obb_adam_plan_t* plan);
+
 /* ---- tile-merge polygon NMS of the DOTA devkit (CPU form, double precision) ---------------------------------------
  * DOTA_devkit/ResultMerge_multi_process.py:62-123 py_cpu_nms_poly_fast over DOTA_devkit/polyiou.cpp:106-128 iou_poly, in
  * double precision without FMA contraction (bit-equal to the reference's g++ build by construction; oracle/poly_ref.py).

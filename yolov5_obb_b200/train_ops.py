@@ -168,3 +168,102 @@ class FusedSGDEMA:
             except Exception:
                 pass
             self._h = None
+
+
+class AdamEntry(ctypes.Structure):
+    """Mirror of y5obb_adam_entry (include/y5obb.h)."""
+    _fields_ = [("p", c_void_p), ("g", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p), ("ema", c_void_p),
+                ("n", c_int64), ("weight_decay", ctypes.c_float), ("group", c_int)]
+
+
+def adam_step_scalars(lr: float, beta1: float, beta2: float, step: float):
+    """(step_size, bias_correction2_sqrt) of torch/optim/adam.py's _multi_tensor_adam (capturable=False) for step count
+    `step`, in its fp64 expression order: -lr / (1 - beta1^t) and (1 - beta2^t)^0.5.  The kernel reads both as fp32, as
+    ATen's foreach kernels read the Python floats."""
+    bias_correction1 = 1 - beta1 ** step
+    bias_correction2 = 1 - beta2 ** step
+    return (lr / bias_correction1) * -1, bias_correction2 ** 0.5
+
+
+class FusedAdamEMA:
+    """optimizer.step() of torch.optim.Adam (train.py --adam, train.py:157-163: coupled L2 weight decay, amsgrad off) +
+    ema.update() as ONE launch.  Parameters, exp_avg and exp_avg_sq are bit-equal to torch's foreach step
+    (tests/test_adam_ema_gpu.py); the EMA is the SGD kernel's (equal to ModelEMA within 1e-5 relative).
+
+    groups, grads, ema_model, weight_decay: as FusedSGDEMA (weight decay on group 1 only).  state: a mapping
+    {parameter: {'step', 'exp_avg', 'exp_avg_sq'}} such as optimizer.state; where it holds every parameter the moments are
+    adopted in place (fp32, contiguous, on the parameter's device) and the step count is theirs, which must be one count for
+    all.  `self.state` is torch.optim.Adam's per-parameter state: the moments the kernel updates and a 'step' that is a view
+    of one CPU fp32 tensor, `step_count`, advanced by one op per step.  step(lr=(lr0, lr1, lr2), betas, eps, ema_decay)."""
+
+    def __init__(self, model, groups, grads, ema_model=None, weight_decay: float = 0.0, state=None):
+        self.device = next(model.parameters()).device
+        ema_sd = dict(ema_model.state_dict()) if ema_model is not None else {}
+        name_of = {id(p): n for n, p in model.named_parameters()}
+        params = [p for plist in groups for p in plist]
+        adopted = [state.get(p) if state is not None else None for p in params]
+        n_have = sum(1 for s in adopted if s)
+        if n_have not in (0, len(params)):
+            raise ValueError(f"FusedAdamEMA: optimizer state holds {n_have} of {len(params)} parameters; it adopts all or none")
+        steps = {float(s["step"]) for s in adopted if s}
+        if len(steps) > 1:
+            raise ValueError(f"FusedAdamEMA: the parameters' Adam step counts differ ({sorted(steps)}); the fused step needs one")
+        self.t = steps.pop() if steps else 0.0
+        self.step_count = torch.full((len(params),), self.t, dtype=torch.float32)
+        self.state, ent, self._keep = {}, [], []
+        i = 0
+        for gi, plist in enumerate(groups):
+            for p in plist:
+                g = grads[p]
+                assert p.dtype == torch.float32 and g.dtype == torch.float32 and p.is_contiguous() and g.is_contiguous()
+                s = adopted[i]
+                if s:
+                    m, v = s["exp_avg"], s["exp_avg_sq"]
+                    for t in (m, v):
+                        if t.dtype != torch.float32 or t.device != p.device or t.shape != p.shape or not t.is_contiguous():
+                            raise ValueError("FusedAdamEMA: adopted moments must be contiguous fp32 tensors shaped and placed "
+                                             "like their parameter")
+                else:
+                    m, v = torch.zeros_like(p), torch.zeros_like(p)
+                self.state[p] = {"step": self.step_count[i], "exp_avg": m, "exp_avg_sq": v}
+                e = ema_sd.get(name_of[id(p)])
+                ent.append(AdamEntry(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(),
+                                     e.data_ptr() if e is not None else None, p.numel(),
+                                     float(weight_decay) if gi == 1 else 0.0, gi))
+                self._keep += [p, g, m, v, e]
+                i += 1
+        if ema_model is not None:  # floating-point buffers (BatchNorm running statistics): EMA only
+            msd = dict(model.state_dict())
+            pnames = set(name_of.values())
+            for k, e in ema_sd.items():
+                if k in pnames or not e.dtype.is_floating_point:
+                    continue
+                b = msd[k]
+                ent.append(AdamEntry(b.data_ptr(), None, None, None, e.data_ptr(), b.numel(), 0.0, -1))
+                self._keep += [b, e]
+        arr = (AdamEntry * len(ent))(*ent)
+        self._h = c_void_p()
+        with torch.cuda.device(self.device):
+            rc = _lib.lib().y5obb_adam_ema_plan_create(arr, len(ent), ctypes.byref(self._h))
+        _lib.check(rc, "y5obb_adam_ema_plan_create")
+
+    def step(self, lr, betas, eps: float, ema_decay: float = 0.0, stream=None):
+        t = self.t + 1.0          # torch advances `step` before it forms the bias corrections
+        b1, b2 = float(betas[0]), float(betas[1])
+        scal = [adam_step_scalars(float(v), b1, b2, t) for v in lr]
+        ss = (ctypes.c_float * 3)(*[s for s, _ in scal])
+        with torch.cuda.device(self.device):
+            rc = _lib.lib().y5obb_adam_ema_plan_run(self._h, ss, b1, b2, scal[0][1], float(eps), float(ema_decay),
+                                                    stream if stream is not None else _lib.stream_ptr(self.device))
+        _lib.check(rc, "y5obb_adam_ema_plan_run")
+        self.step_count.add_(1)   # every parameter's state['step'] at once
+        self.t = t
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            try:
+                _lib.lib().y5obb_adam_ema_plan_destroy(h)
+            except Exception:
+                pass
+            self._h = None

@@ -7,7 +7,8 @@
     optimizer.step(); optimizer.zero_grad(); ema.update(model)   # train.py:336-342
 
 Parameter groups follow train.py:148-162 (BatchNorm weights: no decay; other weights: weight decay; biases),
-SGD with Nesterov momentum (train.py:158), ModelEMA as utils/torch_utils.py:284-314.
+SGD with Nesterov momentum (train.py:158) or, with adam=True, Adam (train.py --adam, train.py:157-163),
+ModelEMA as utils/torch_utils.py:284-314.
 The device computes in bf16 with fp32 accumulation and fp32 master weights: no loss scaling is needed (the reference's
 GradScaler exists for fp16 autocast, train.py:246,333-337)."""
 import math
@@ -101,7 +102,7 @@ class TrainStep:
     """model: yolov5_obb_b200.yolo.Model on a CUDA device, in train() mode.  step(imgs, targets) -> (loss, loss_items)."""
 
     def __init__(self, model, hyp: Optional[dict] = None, batch_size: int = 16, imgsz: int = 1024, ema: bool = True,
-                 warmup_iters: int = 0, multi_scale: bool = False, seed: Optional[int] = None):
+                 warmup_iters: int = 0, multi_scale: bool = False, seed: Optional[int] = None, adam: bool = False):
         """warmup_iters > 0: the warm-up of train.py:305-316 over that many iterations (the reference uses
         max(round(warmup_epochs * batches_per_epoch), 1000)): every group's lr is interpolated from 0 (biases: from
         hyp['warmup_bias_lr']) to lr0 and the momentum from hyp['warmup_momentum'] to hyp['momentum'].
@@ -113,7 +114,13 @@ class TrainStep:
         `random` stays the augmentation's (augment.DeviceAugmentLoader), as in the reference with dataloader workers,
         where the main process draws nothing else from it.  The constructor reserves one training arena
         (Model.reserve_train_arena) for batch_size images of the largest drawable size, assuming imgsz x imgsz batches
-        (no --rect), so an out-of-memory error shows at start-up.  `last_shape` is the (h, w) the last step trained at."""
+        (no --rect), so an out-of-memory error shows at start-up.  `last_shape` is the (h, w) the last step trained at.
+
+        adam=True: train.py --adam.  The optimizer is torch.optim.Adam(g0, lr=lr0, betas=(momentum, 0.999)) with g1 (weight
+        decay) and g2 added as for SGD; Adam groups have no 'momentum', so the warm-up moves only the learning rates.  The
+        fused step (below) keeps torch's own per-parameter state in optimizer.state, so optimizer.state_dict() is the
+        reference's checkpoint format, and after optimizer.load_state_dict() the next step continues from the loaded
+        moments and step count."""
         self.model = model
         self.hyp = dict(HYP_FINETUNE_DOTA if hyp is None else hyp)
         nbs = 64
@@ -143,7 +150,12 @@ class TrainStep:
             if hasattr(model, "_bump_generation"):
                 model._bump_generation()
         g0, g1, g2 = param_groups(model)
-        self.optimizer = torch.optim.SGD(g0, lr=self.hyp["lr0"], momentum=self.hyp["momentum"], nesterov=True, foreach=True)
+        self.adam = bool(adam)
+        if self.adam:
+            self.optimizer = torch.optim.Adam(g0, lr=self.hyp["lr0"], betas=(self.hyp["momentum"], 0.999), foreach=True)
+        else:
+            self.optimizer = torch.optim.SGD(g0, lr=self.hyp["lr0"], momentum=self.hyp["momentum"], nesterov=True,
+                                             foreach=True)
         self.optimizer.add_param_group({"params": g1, "weight_decay": self.hyp["weight_decay"]})
         self.optimizer.add_param_group({"params": g2})
         self.ema = ModelEMA(model) if ema else None
@@ -154,9 +166,11 @@ class TrainStep:
         self.optimizer.zero_grad(set_to_none=True)
         # optimizer.step() + ema.update() as ONE kernel (csrc/sgd_ema.cu, SURVEY 8f rank 1) whenever every batch ends with an
         # optimizer step (accumulate == 1: the gradient of the step is exactly the backward plan's flat buffer).  With gradient
-        # accumulation torch.optim.SGD + the foreach EMA below stay in charge.  Y5OBB_FUSED_SGD=0 forces the torch path.
+        # accumulation torch.optim.SGD / Adam + the foreach EMA below stay in charge.  Y5OBB_FUSED_SGD=0 forces the torch path
+        # for either optimizer.
         import os
         self._fused = None
+        self._fused_state = None
         self._use_fused = (self.accumulate == 1 and os.environ.get("Y5OBB_FUSED_SGD", "1") != "0"
                            and next(model.parameters()).is_cuda and hasattr(model, "_bump_generation"))
         if self.multi_scale:
@@ -297,27 +311,49 @@ class TrainStep:
         """train.py:336-342 (optimizer.step, zero_grad, ema.update) as one launch over a device-resident tensor table.
         Gradients are read in place from the backward plan's flat fp32 buffer (all-reduced in place first when N > 1);
         learning rates / momentum are taken from optimizer.param_groups every step, so warm-up schedules that edit them
-        (train.py:305-316) keep working; the momentum buffers are registered in optimizer.state for checkpoints."""
-        from .train_ops import FusedSGDEMA
+        (train.py:305-316) keep working; the momentum buffers are registered in optimizer.state for checkpoints.
+        Adam: lr, betas and eps are read the same way, and optimizer.state holds torch's exp_avg / exp_avg_sq / step, which
+        the kernel updates in place.  optimizer.load_state_dict() replaces optimizer.state, so a new state object means a
+        checkpoint was loaded: the table is rebuilt on the loaded tensors."""
+        from .train_ops import FusedAdamEMA, FusedSGDEMA
         model = self.model
         plan = model._last_train_engine._bwd
         if self.world > 1:
             dist.all_reduce(plan.flat, op=dist.ReduceOp.SUM)
         key = plan.flat if plan.arena is not None else plan   # (an arena's flat buffer is shared by every shape)
-        if self._fused is None or self._fused_plan is not key:
-            groups = [g["params"] for g in self.optimizer.param_groups]
-            self._fused = FusedSGDEMA(model, groups, plan.pgrad, self.ema.ema if self.ema is not None else None,
+        ema = self.ema.ema if self.ema is not None else None
+        opt = self.optimizer
+        if self.adam:
+            if self._fused is None or self._fused_plan is not key or self._fused_state is not opt.state:
+                groups = [g["params"] for g in opt.param_groups]
+                self._fused = FusedAdamEMA(model, groups, plan.pgrad, ema, weight_decay=self.hyp["weight_decay"],
+                                           state=opt.state)
+                self._fused_plan = key
+                for p, s in self._fused.state.items():
+                    opt.state[p] = s
+                self._fused_state = opt.state
+        elif self._fused is None or self._fused_plan is not key:
+            groups = [g["params"] for g in opt.param_groups]
+            self._fused = FusedSGDEMA(model, groups, plan.pgrad, ema,
                                       weight_decay=self.hyp["weight_decay"], momentum_buffers=getattr(self, "_mom", None))
             self._mom = self._fused.mom
             self._fused_plan = key
             for p, m in self._fused.mom.items():
-                self.optimizer.state[p]["momentum_buffer"] = m
-        g = self.optimizer.param_groups
+                opt.state[p]["momentum_buffer"] = m
+        g = opt.param_groups
+        if self.adam:
+            betas, eps = g[0]["betas"], g[0]["eps"]
+            if any(tuple(x["betas"]) != tuple(betas) or x["eps"] != eps for x in g[1:]):
+                raise ValueError("the fused Adam step needs one (betas, eps) for every parameter group; "
+                                 "set Y5OBB_FUSED_SGD=0 to step per group with torch.optim.Adam")
         d = 0.0
         if self.ema is not None:
             self.ema.updates += 1
             d = self.ema.decay(self.ema.updates)
-        self._fused.step((g[0]["lr"], g[1]["lr"], g[2]["lr"]), g[0]["momentum"], d)
+        if self.adam:
+            self._fused.step((g[0]["lr"], g[1]["lr"], g[2]["lr"]), betas, eps, d)
+        else:
+            self._fused.step((g[0]["lr"], g[1]["lr"], g[2]["lr"]), g[0]["momentum"], d)
         self.optimizer.zero_grad(set_to_none=True)
         model._bump_generation()   # parameters changed through raw pointers: inference plans must re-fold them
         if self.ema is not None and hasattr(self.ema.ema, "_bump_generation"):
