@@ -120,6 +120,8 @@ typedef struct y5obb_conv y5obb_conv_t;
 #define Y5OBB_CONV_NO_PDL 32       /* flags: plain stream-ordered launch (default: programmatic dependent launch - the kernel's
                                       prologue overlaps the previous kernel's tail and it waits, griddepcontrol.wait, before its
                                       first global-memory access; also switched off by the environment variable Y5OBB_NO_PDL=1) */
+#define Y5OBB_CONV_ONE_CTA 64      /* flags: one CTA per SM even for N tiles <= 96 (default: two when the plan fits half of
+                                      the shared memory; debug / A-B comparison) */
 
 typedef struct {
   const void* in;            /* bf16 NHWC slice */
@@ -166,6 +168,9 @@ int y5obb_conv_create(const y5obb_conv_desc* desc, y5obb_conv_t** out);
 int y5obb_conv_run(const y5obb_conv_t* conv, void* stream);
 int y5obb_conv_info(const y5obb_conv_t* conv, double* flops, double* hbm_bytes, int* grid, int* block_n,
                     int* block_k, int* stages);
+/* The rest of the launch plan: CTAs resident per SM (1 or 2), weights resident in shared memory (0/1), row-shift A stages
+   (0/1) and (tap, K-chunk) units per pipeline stage.  Any pointer may be NULL. */
+int y5obb_conv_schedule(const y5obb_conv_t* conv, int* ctas_per_sm, int* resident, int* rowshift, int* group);
 void y5obb_conv_destroy(y5obb_conv_t* conv);
 
 /* ---- HBM-bound helpers around the conv stack -------------------------------------------------

@@ -39,6 +39,7 @@ PROTOTYPES = {
     "y5obb_conv_run": (c_int, [c_void_p, c_void_p]),
     "y5obb_conv_info": (c_int, [c_void_p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]
                         + [ctypes.POINTER(c_int)] * 4),
+    "y5obb_conv_schedule": (c_int, [c_void_p] + [ctypes.POINTER(c_int)] * 4),
     "y5obb_conv_destroy": (None, [c_void_p]),
     "y5obb_loss_workspace_bytes": (c_size_t, [c_void_p]),
     "y5obb_loss_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -121,6 +121,7 @@ class WindowView:
 
 
 NO_ROWSHIFT, NO_RESIDENT, NO_PAIRW, BIAS_HALVED = 1, 2, 4, 8
+ONE_CTA = 64   # one CTA per SM for every instantiation (A/B comparison of the two-CTA plans)
 
 
 class Conv:
@@ -187,8 +188,10 @@ class Conv:
         g, bn, bk, st = c_int(), c_int(), c_int(), c_int()
         _lib.lib().y5obb_conv_info(self._h, ctypes.byref(fl), ctypes.byref(by), ctypes.byref(g), ctypes.byref(bn),
                                    ctypes.byref(bk), ctypes.byref(st))
+        cta, res, rs, grp = c_int(), c_int(), c_int(), c_int()
+        _lib.lib().y5obb_conv_schedule(self._h, ctypes.byref(cta), ctypes.byref(res), ctypes.byref(rs), ctypes.byref(grp))
         return dict(flops=fl.value, hbm_bytes=by.value, grid=g.value, block_n=bn.value, block_k=bk.value,
-                    stages=st.value)
+                    stages=st.value, ctas_per_sm=cta.value, resident=res.value, rowshift=rs.value, group=grp.value)
 
     def __del__(self):
         h = getattr(self, "_h", None)

@@ -13,7 +13,7 @@
 //             stride-2 convs use the tensor map's element strides (or the pixel-pair view).
 //   W tile  = 2-D TMA box {BK, NI} of weights packed [tap][Cout_pad][Cin_pad] (K-major).
 //   Both land in 32/64/128-byte swizzled K-major layouts that wgmma reads through shared-memory descriptors.
-// One persistent CTA per SM, three warpgroups: two consumers (pixel rows 0-63 and 64-127 of the tile, each issuing
+// Persistent CTAs (one per SM, or two for N tiles <= 96, see Occupancy), three warpgroups: two consumers (pixel rows 0-63 and 64-127 of the tile, each issuing
 // m64nNIk16 wgmma over the whole N tile and running the epilogue of its rows) and a producer whose first warp issues the
 // TMA loads.  setmaxnreg moves the producer's registers to the consumers (up to 128 fp32 accumulators per thread).  The producer
 // runs ahead through a ring of pipeline stages, so the next tile's operands arrive while the epilogue of this one runs.
@@ -39,9 +39,28 @@ constexpr int BM = 128;  // output pixels per tile
 constexpr int MAX_STAGES = 16;
 constexpr int CONSUMER_WARPS = 8;                        // two warpgroups of 64 pixel rows each
 constexpr int NUM_THREADS = 32 * (CONSUMER_WARPS + 4);   // + the producer warpgroup (one warp issues the TMA loads)
-constexpr int STG_PITCH = 68;                            // fp32 per staged row: 64 columns + 4 (spreads the banks)
-constexpr int STG_BYTES = (16 * STG_PITCH + 16) * 4;     // per consumer warp: 16 rows x 64 columns, then 16 theta indices
 constexpr int SMEM_TOTAL = 224 * 1024;                   // dynamic shared memory we ask for at most (227 KB is the H100 cap)
+// Two CTAs per SM: 2 x (112 KB dynamic + 1 KB static + 1 KB per-block reservation) = 228 KB, exactly the H100's shared
+// memory per SM, with no headroom.  The static part is the mbarriers padded to 1 KB by smem_raw's __align__(1024).  Any
+// added static shared memory makes the occupancy check in y5obb_conv_create send every narrow layer back to one CTA
+// (correct, but slower); y5obb_conv_schedule and tests/test_conv_schedule_gpu.py expose that.
+constexpr int SMEM_PAIR = 112 * 1024;
+
+// Epilogue staging per consumer warp: 16 rows x min(NI, 64) fp32 columns, each row padded by 4 (spreads the banks), then
+// 16 theta indices.
+__host__ __device__ constexpr int stg_cols(int ni) { return ni < 64 ? ni : 64; }
+__host__ __device__ constexpr int stg_pitch(int ni) { return stg_cols(ni) + 4; }
+__host__ __device__ constexpr int stg_bytes(int ni) { return (16 * stg_pitch(ni) + 16) * 4; }
+
+// Instantiations with NI <= 96 run two CTAs per SM: 2 x 384 threads at 80 registers each, of which setmaxnreg gives the
+// producer warpgroup 32 and the consumers 104 (128 * 32 + 256 * 104 = 384 * 80).  Wider ones keep the SM to themselves,
+// with 40 / 232 (up to 128 fp32 accumulators per consumer thread).
+template <int NI>
+struct Occupancy {
+  static constexpr int CTAS = NI <= 96 ? 2 : 1;
+  static constexpr int PRODUCER_REGS = CTAS == 2 ? 32 : 40;
+  static constexpr int CONSUMER_REGS = CTAS == 2 ? 104 : 232;
+};
 
 enum Mode : int { MODE_CONV = 0, MODE_DETECT = 1 };
 
@@ -147,7 +166,8 @@ template <int NI>
 __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg, const float* bias_s,
                                          int row0, int lane) {
   const int q = lane & 3, r = lane >> 2;
-  float* theta_s = stg + 16 * STG_PITCH;
+  constexpr int PITCH = stg_pitch(NI), VECS = stg_cols(NI) / 8;  // 8-column vectors per staged row
+  float* theta_s = stg + 16 * PITCH;
   const bool det = p.mode == MODE_DETECT;
   const int nvalid = min(p.BN, (det ? p.det_no : p.Cout - c.n0));
   const int nfix = p.det_no - 180;  // Detect: 5 + nc leading columns, then the theta bins
@@ -209,20 +229,20 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
             v0 += b0;
             v1 += b1;
           }
-          *reinterpret_cast<float2*>(stg + (r + 8 * i) * STG_PITCH + (col - cb)) = make_float2(v0, v1);
+          *reinterpret_cast<float2*>(stg + (r + 8 * i) * PITCH + (col - cb)) = make_float2(v0, v1);
         }
       }
     }
     __syncwarp();
     // (2) 16 rows x (up to) 64 columns leave in vectors
     if (!det) {
-      for (int v = lane; v < 16 * 8; v += 32) {
-        const int row = v >> 3, col = cb + (v & 7) * 8;
+      for (int v = lane; v < 16 * VECS; v += 32) {
+        const int row = v / VECS, col = cb + (v % VECS) * 8;
         const int tr = row0 + row;
         const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
         const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
         if (col >= nvalid || h >= p.Hout || w >= p.Wout) continue;
-        const float* sp = stg + row * STG_PITCH + (col - cb);
+        const float* sp = stg + row * PITCH + (col - cb);
         const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
         float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
         const int ch = c.n0 + col;
@@ -265,7 +285,7 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
         const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
         const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
         if (col >= ncols || h >= p.Hout || w >= p.Wout) continue;
-        const float4 x = *reinterpret_cast<const float4*>(stg + row * STG_PITCH + (col - cb));
+        const float4 x = *reinterpret_cast<const float4*>(stg + row * PITCH + (col - cb));
         float f[4] = {x.x, x.y, x.z, x.w};
         if (p.det_decode) {
 #pragma unroll
@@ -297,7 +317,7 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
 }
 
 template <int NI>
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_wgmma_kernel(const __grid_constant__ ConvK p) {
+__global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_kernel(const __grid_constant__ ConvK p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
   __shared__ __align__(8) uint64_t empty_bar[MAX_STAGES];
@@ -309,7 +329,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_wgmma_kernel(const __grid
   const uint32_t unit_bytes = p.a_bytes + (uint32_t)p.b_per_stage * p.b_stage_bytes;
   const uint32_t stage_bytes = unit_bytes * (uint32_t)p.group;
   uint8_t* stg_all = smem + (size_t)p.stages * stage_bytes;
-  float* bias_s = reinterpret_cast<float*>(stg_all + (size_t)CONSUMER_WARPS * STG_BYTES);
+  float* bias_s = reinterpret_cast<float*>(stg_all + (size_t)CONSUMER_WARPS * stg_bytes(NI));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -336,7 +356,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_wgmma_kernel(const __grid
 
   if (warp >= CONSUMER_WARPS) {
     // ===================== TMA producer =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Occupancy<NI>::PRODUCER_REGS));
     if (warp == CONSUMER_WARPS && ptx::elect_one()) {
       if (p.b_resident) {  // all weight tiles, once: tile (tap, kc) at smem_res + (tap * kchunks + kc) * b_stage_bytes
         const int ntile = p.KH * p.KW * p.kchunks;
@@ -393,13 +413,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_wgmma_kernel(const __grid
   }
 
   // ===================== consumers: warpgroup wg owns pixel rows [64 wg, 64 wg + 64) of every tile =====================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Occupancy<NI>::CONSUMER_REGS));
   for (int i = threadIdx.x; i < p.cout_pad + 32; i += 32 * CONSUMER_WARPS) bias_s[i] = __ldg(p.bias + i);
   asm volatile("bar.sync 1, %0;" ::"n"(32 * CONSUMER_WARPS) : "memory");
   if (p.b_resident) ptx::mbar_wait(&wres_bar, 0u);
 
   const int wg = warp >> 2;
-  float* stg = reinterpret_cast<float*>(stg_all + (size_t)warp * STG_BYTES);
+  float* stg = reinterpret_cast<float*>(stg_all + (size_t)warp * stg_bytes(NI));
   // descriptors differ only in the 14-bit (address >> 4) field of the low word
   const uint64_t desc0 = ptx::make_kmajor_desc(0u, (uint32_t)p.BK * 2u);
   const uint32_t hi = (uint32_t)(desc0 >> 32);
@@ -500,6 +520,7 @@ CUtensorMapSwizzle swizzle_for(int bk) {
 int instr_n(int bn) { return bn <= 16 ? 16 : (bn + 31) / 32 * 32; }
 
 typedef void (*KernelFn)(ConvK);
+int ctas_for(int ni) { return ni <= 96 ? 2 : 1; }  // Occupancy<NI>::CTAS
 KernelFn kernel_for(int ni) {
   switch (ni) {
     case 16: return conv_wgmma_kernel<16>;
@@ -519,6 +540,7 @@ struct ConvObj {
   ConvK k;
   KernelFn fn;
   int grid;
+  int ctas_per_sm;   // 1, or 2 for the NI <= 96 instantiations when their plan fits half of the shared memory
   int threads;
   size_t smem;
   double flops;      // algorithmic 2*MACs
@@ -622,7 +644,8 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
   int a_rows = 0;
   size_t stage_bytes = 0;
   const size_t bias_bytes = align_up((size_t)(cout_pad + 32) * 4, 128);  // the bias lives in shared memory behind the staging buffers
-  const size_t SMEM_BUDGET = (size_t)SMEM_TOTAL - 1024 - (size_t)CONSUMER_WARPS * STG_BYTES - bias_bytes;
+  const size_t fixed_bytes = 1024 + (size_t)CONSUMER_WARPS * stg_bytes(ni) + bias_bytes;  // alignment slack, staging, bias
+  size_t SMEM_BUDGET = 0;  // for the operand ring and the resident weights: set per CTAs-per-SM choice below
   // Row-shift mode (stride-1 convs with KH > 1): an 8 x 16 pixel tile whose A stage holds Ht + KH - 1 image
   // rows; the KH vertical taps read the same stage at row offsets that are whole 8-row swizzle groups, so each
   // input row crosses L2 -> shared memory (Ht + KH - 1) / Ht times per kw instead of KH times.  Taken when the
@@ -676,9 +699,53 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     return k.stages >= (rowshift ? 3 : 2);
   };
   const bool want_rowshift = d->stride == 1 && d->KH > 1 && Wout >= 8 && !(d->flags & Y5OBB_CONV_NO_ROWSHIFT);
-  if (!((want_rowshift && plan(true)) || plan(false))) {
+  // Row shift sums the (tap, K-chunk) terms in another order than one load per tap.  That order is fixed here, by the
+  // full-SM plan with 64-column staging, and every plan below keeps it: the schedule never changes a result bit.
+  SMEM_BUDGET = (size_t)SMEM_TOTAL - (1024 + (size_t)CONSUMER_WARPS * stg_bytes(64) + bias_bytes);
+  const bool rowshift_order = want_rowshift && plan(true);
+  // Narrow instantiations share the SM between two CTAs when the layer's plan fits half of the shared memory: while one
+  // CTA runs a tile's epilogue (or waits on its residual loads) the other's MMAs and loads go on.
+  auto plan_for = [&](int ctas) -> bool {
+    const size_t cap = ctas == 2 ? (size_t)SMEM_PAIR : (size_t)SMEM_TOTAL;
+    if (cap <= fixed_bytes) return false;
+    SMEM_BUDGET = cap - fixed_bytes;
+    return plan(rowshift_order);
+  };
+  o->ctas_per_sm = 1;
+  if (ctas_for(ni) == 2 && !(d->flags & Y5OBB_CONV_ONE_CTA) && plan_for(2)) o->ctas_per_sm = 2;
+  if (o->ctas_per_sm == 1 && !plan_for(1)) {
     delete o;
     return Y5OBB_EINVAL;
+  }
+  static bool attr_set[257] = {};  // per instantiation (one per NI)
+  if (!attr_set[ni]) {
+    // all of the unified L1 / shared memory as shared memory, so that two 112 KB CTAs fit beside each other
+    cudaError_t e = cudaFuncSetAttribute(o->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(o->fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e != cudaSuccess) {
+      delete o;
+      return cuda_fail(e);
+    }
+    attr_set[ni] = true;
+  }
+  auto smem_of_plan = [&]() { return k.b_res_bytes + (size_t)k.stages * stage_bytes + fixed_bytes; };
+  o->smem = smem_of_plan();
+  if (o->ctas_per_sm == 2) {  // the occupancy calculator has the last word; a plan that would run alone takes the full-SM plan
+    int blocks = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, o->fn, NUM_THREADS, o->smem);
+    if (e != cudaSuccess) {
+      delete o;
+      return cuda_fail(e);
+    }
+    if (blocks < 2) {
+      o->ctas_per_sm = 1;
+      if (!plan_for(1)) {
+        delete o;
+        return Y5OBB_EINVAL;
+      }
+      o->smem = smem_of_plan();
+    }
   }
   {
     const char* e = getenv("Y5OBB_NO_PDL");
@@ -774,21 +841,11 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     }
   }
   const int total = k.n_tiles_m * k.n_tiles_n;
-  o->grid = std::min(total, sm_count());
+  o->grid = std::min(total, o->ctas_per_sm * sm_count());
   if (k.b_resident && k.n_tiles_n > 1) o->grid = o->grid / k.n_tiles_n * k.n_tiles_n;  // one N tile per CTA (resident weights)
   o->threads = NUM_THREADS;
-  o->smem = k.b_res_bytes + (size_t)k.stages * stage_bytes + (size_t)CONSUMER_WARPS * STG_BYTES + bias_bytes + 1024;
   o->flops = 2.0 * d->B * Hout * Wout * (double)d->Cout * d->Cin * d->KH * d->KW;
   o->hbm_bytes = 2.0 * d->B * ((double)d->Hin * d->Win * (d->hbm_cin ? d->hbm_cin : d->Cin) + (double)Hout * Wout * d->Cout * (d->res ? 2 : 1));
-  static bool attr_set[257] = {};
-  if (!attr_set[ni]) {
-    cudaError_t e = cudaFuncSetAttribute(o->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
-    if (e != cudaSuccess) {
-      delete o;
-      return cuda_fail(e);
-    }
-    attr_set[ni] = true;
-  }
   *out = reinterpret_cast<y5obb_conv_t*>(o);
   return Y5OBB_OK;
 }
@@ -822,6 +879,16 @@ int y5obb_conv_info(const y5obb_conv_t* conv, double* flops, double* hbm_bytes, 
   if (block_n) *block_n = o->k.BN;
   if (block_k) *block_k = o->k.BK;
   if (stages) *stages = o->k.stages;
+  return Y5OBB_OK;
+}
+
+int y5obb_conv_schedule(const y5obb_conv_t* conv, int* ctas_per_sm, int* resident, int* rowshift, int* group) {
+  if (!conv) return Y5OBB_EINVAL;
+  const ConvObj* o = reinterpret_cast<const ConvObj*>(conv);
+  if (ctas_per_sm) *ctas_per_sm = o->ctas_per_sm;
+  if (resident) *resident = o->k.b_resident;
+  if (rowshift) *rowshift = o->k.rowshift;
+  if (group) *group = o->k.group;
   return Y5OBB_OK;
 }
 
