@@ -92,12 +92,12 @@ def build_targets(p, targets, anchors, stride, anchor_t, na=3):
 def compute_loss(p, targets, anchors, stride, hyp, nc):
     """loss.py:122-192.  p: list of [B, na, H, W, no] tensors (requires_grad for the backward check).
     Returns (loss[1], items[4])."""
-    dev = targets.device
-    lcls, lbox, lobj, ltheta = (torch.zeros(1, device=dev) for _ in range(4))
+    dev, dt = targets.device, p[0].dtype   # fp64 predictions: CIoU, BCE and autograd in fp64, matching still in fp32
+    lcls, lbox, lobj, ltheta = (torch.zeros(1, device=dev, dtype=dt) for _ in range(4))
     tcls, tbox, indices, anch, tcsl = build_targets(p, targets, anchors, stride, hyp["anchor_t"], anchors.shape[1])
     cp, cn = 1.0 - 0.5 * hyp.get("label_smoothing", 0.0), 0.5 * hyp.get("label_smoothing", 0.0)
     balance = {3: [4.0, 1.0, 0.4]}.get(len(p), [4.0, 1.0, 0.25, 0.06, 0.02])
-    pw = lambda k: torch.tensor([hyp[k]], device=dev)
+    pw = lambda k: torch.tensor([hyp[k]], device=dev, dtype=dt)
     for i, pi in enumerate(p):
         b, a, gj, gi = indices[i]
         tobj = torch.zeros_like(pi[..., 0])
@@ -107,7 +107,7 @@ def compute_loss(p, targets, anchors, stride, hyp, nc):
             pxy = ps[:, :2].sigmoid() * 2 - 0.5
             pwh = (ps[:, 2:4].sigmoid() * 2) ** 2 * anch[i]
             pbox = torch.cat((pxy, pwh), 1)
-            iou = bbox_ciou(pbox.T, tbox[i])
+            iou = bbox_ciou(pbox.T, tbox[i].to(dt))
             lbox = lbox + (1.0 - iou).mean()
             tobj[b, a, gj, gi] = iou.detach().clamp(0).type(tobj.dtype)  # gr = 1.0; sequential last-writer-wins on CPU
             ci = 5 + nc

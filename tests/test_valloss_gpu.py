@@ -11,7 +11,7 @@ import torch
 from oracle import loss_ref, model_ref
 from tests import vallossgen as VG
 from tests.losscases import FakeModel
-from tests.lossgen import synth_targets
+from tests.lossgen import boundary_targets, synth_targets
 from yolov5_obb_b200 import _lib, general
 from yolov5_obb_b200.loss import ComputeLoss, LossHead, compact_csl_index
 from yolov5_obb_b200.val import Validator
@@ -95,11 +95,14 @@ def test_exact_b16_1024(size):
 
 def test_exact_320x256_layouts_and_duplicates():
     """P5 of a 256 x 320 input has 80 cells per (image, anchor): the 256-cell obj blocks straddle anchors.  Rows repeated
-    verbatim land in the same cells (the last writer wins tobj); every target layout."""
+    verbatim land in the same cells (the last writer wins tobj); every target layout.  Then targets on build_targets'
+    boundaries (tests/lossgen.boundary_targets)."""
     B = 2
     tg = torch.from_numpy(synth_targets(B, 40, 256, seed=12))
     tg = torch.cat([tg, tg[5:9], tg[5:6]])
     _assert_exact(B, 256, 320, CHANNELS["s"], tg, seed=6, cols=(187, 8, 7))
+    _assert_exact(B, 256, 320, CHANNELS["s"], torch.from_numpy(boundary_targets(B, 256, 320, seed=13)), seed=6,
+                  cols=(187, 8, 7))
 
 
 def test_exact_empty_targets():

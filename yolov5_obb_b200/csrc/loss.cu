@@ -191,9 +191,14 @@ __device__ __forceinline__ D4 operator/(const D4& a, const D4& b) {
 __device__ __forceinline__ D4 dscale(const D4& a, float s) {
   return D4{a.v * s, {a.d[0] * s, a.d[1] * s, a.d[2] * s, a.d[3] * s}};
 }
-__device__ __forceinline__ D4 dmin(const D4& a, const D4& b) { return a.v <= b.v ? a : b; }
-__device__ __forceinline__ D4 dmax(const D4& a, const D4& b) { return a.v >= b.v ? a : b; }
-__device__ __forceinline__ D4 dclamp0(const D4& a) { return a.v > 0.f ? a : dconst(0.f); }
+// torch's rules at ties: minimum / maximum give each side half the derivative, clamp(0) passes it at exactly 0.  Zero box
+// logits put the predicted box at (cell + 0.5, anchor), so a target of the anchor's width centred on a cell ties on both edges.
+__device__ __forceinline__ D4 dtie(const D4& a, const D4& b) {
+  return D4{a.v, {0.5f * (a.d[0] + b.d[0]), 0.5f * (a.d[1] + b.d[1]), 0.5f * (a.d[2] + b.d[2]), 0.5f * (a.d[3] + b.d[3])}};
+}
+__device__ __forceinline__ D4 dmin(const D4& a, const D4& b) { return a.v < b.v ? a : (b.v < a.v ? b : dtie(a, b)); }
+__device__ __forceinline__ D4 dmax(const D4& a, const D4& b) { return a.v > b.v ? a : (b.v > a.v ? b : dtie(a, b)); }
+__device__ __forceinline__ D4 dclamp0(const D4& a) { return a.v >= 0.f ? a : dconst(0.f); }
 __device__ __forceinline__ D4 datan(const D4& a) {
   const float g = 1.0f / (1.0f + a.v * a.v);
   return D4{atanf(a.v), {a.d[0] * g, a.d[1] * g, a.d[2] * g, a.d[3] * g}};
