@@ -259,6 +259,12 @@ int y5obb_loss_forward_head(const y5obb_loss_desc* desc, const y5obb_loss_head* 
 int y5obb_rbox2poly_f32(const float* rboxes5, float* polys8, int64_t n, void* stream);
 int y5obb_poly2hbb_f32(const float* polys8, float* hbb4, int64_t n, void* stream);
 int y5obb_scale_polys_f32(float* polys8, int64_t n, float pad_x, float pad_y, float gain, void* stream);
+/* rbox2poly followed by scale_polys for the packed NMS output of a whole batch, as detect.py:129-147 / val.py:226-232 apply
+ * them per image: rows7 [B, max_det, 7] (cx, cy, l, s, theta, conf, cls), counts [>= B] int64 valid rows per image,
+ * pad_gain3 [B, 3] fp32 (pad_x, pad_y, gain) per image -> polys8 [B, max_det, 8] in source-image pixels.  The same separately
+ * rounded fp32 operations as the two calls above, so the result equals calling them in turn; rows >= counts[b] are zero. */
+int y5obb_scale_polys_batched_f32(const float* rows7, const int64_t* counts, const float* pad_gain3, int B, int max_det,
+                                  float* polys8, void* stream);
 /* poly2rbox (utils/rboxs_utils.py:39-81, whose arithmetic is cv2.minAreaRect): [n,8] fp32 corner points ->
  * [n,5] fp64 (cx, cy, long edge, short edge, theta); theta in [-pi/2, pi/2) with pi = 3.141592 (use_pi) or degrees in [0, 180) */
 int y5obb_poly2rbox(const float* polys8, double* rbox5, int64_t n, int use_pi, void* stream);
@@ -413,6 +419,40 @@ size_t y5obb_poly_nms_workspace_bytes(int64_t n);
 int y5obb_poly_nms_f64(const double* dets9, int64_t n, double thresh, int64_t* keep_out, int64_t* n_keep_out, void* workspace,
                        size_t workspace_bytes, void* stream);
 int y5obb_poly_iou_pairs_f64(const double* p8, const double* q8, double* iou_out, int64_t n, void* stream);
+
+/* ---- image files of any size: letterbox straight into the stem input ------------------------------------------------------
+ * y5obb_letterbox_s2d_u8 replaces the host front end of detect.py and val.py for a batch of B images of different sizes:
+ * utils/datasets.py:217-229 (LoadImages.__next__) and :585-590,662-663,702-720 (LoadImagesAndLabels.__getitem__,
+ * load_image_label), i.e. cv2.resize to new_w x new_h, utils/augmentations.py:92-128 letterbox's copyMakeBorder with 114,
+ * `transpose((2, 0, 1))[::-1]` and the caller's `/ 255`.
+ * src: the images as cv2.imread returns them (uint8 HWC BGR), packed back to back; image b starts at byte src_off.
+ * desc_dev: B descriptors followed by the per-image tables, one device buffer of desc_bytes bytes; desc_host: the same bytes
+ * in host memory, read before the launch to refuse descriptors that reach outside src, the tables or the Hp x Wp image.
+ * Table offsets xtab / ytab count 32-bit words from the start of the buffer.
+ *   Y5OBB_LB_COPY      new size == source size, no resampling.
+ *   Y5OBB_LB_LINEAR    cv2.INTER_LINEAR, 8-bit fixed point.  Per destination column two words: the first source column, and the
+ *                      coefficient pair saturate_cast<short>((1 - fx) * 2048) | saturate_cast<short>(fx * 2048) << 16; rows the same.
+ *   Y5OBB_LB_AREA_INT  cv2.INTER_AREA by integer factors kx, ky (and INTER_LINEAR when both are exactly 2, which OpenCV
+ *                      resamples as INTER_AREA): (sum + 2) >> 2 for 2x2, else round-half-even of (float)sum * inv_area.
+ *   Y5OBB_LB_AREA      cv2.INTER_AREA by a fractional factor, shrinking.  Per axis n + 1 first-tap indices, then per tap two
+ *                      words (source index, fp32 weight), in OpenCV's table order.
+ * Output: y5obb_stem_s2d_u8's layout [B, Hp/2, Wp/2 + 2*pad_cols, 16] bf16; pixel (y, x) is 114 outside
+ * [top, top + new_h) x [left, left + new_w), else the resampled source pixel in RGB order.  The pad_cols columns are not
+ * written.  The resampled bytes equal the installed OpenCV's bit for bit (oracle/letterbox_ref.py restates them). */
+enum { Y5OBB_LB_COPY = 0, Y5OBB_LB_LINEAR = 1, Y5OBB_LB_AREA_INT = 2, Y5OBB_LB_AREA = 3 };
+typedef struct {
+  int64_t src_off;           /* byte offset of the image in src */
+  int32_t h0, w0;            /* source size */
+  int32_t new_h, new_w;      /* resampled size */
+  int32_t top, left;         /* where the resampled image starts in the Hp x Wp letterboxed image */
+  int32_t mode;              /* Y5OBB_LB_* */
+  int32_t kx, ky;            /* Y5OBB_LB_AREA_INT: the block */
+  float inv_area;            /* Y5OBB_LB_AREA_INT: 1.f / (kx * ky) */
+  int32_t xtab, ytab;        /* word offsets of the column / row table */
+  int32_t reserved[2];
+} y5obb_letterbox_desc;      /* 64 bytes */
+int y5obb_letterbox_s2d_u8(const uint8_t* src, int64_t src_bytes, const void* desc_dev, const y5obb_letterbox_desc* desc_host,
+                           int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16, int pad_cols, void* stream);
 
 /* ---- whole-scene inference: tile input and tile-merge (DOTA scenes larger than one tile) --------------------------------
  * The reference's route (README.md:24-26): DOTA_devkit/ImgSplit_multi_process.py:226-273 cuts the scene into subsize^2 tiles

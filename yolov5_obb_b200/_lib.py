@@ -49,6 +49,7 @@ PROTOTYPES = {
     "y5obb_rbox2poly_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "y5obb_poly2hbb_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "y5obb_scale_polys_f32": (c_int, [c_void_p, c_int64, c_float, c_float, c_float, c_void_p]),
+    "y5obb_scale_polys_batched_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "y5obb_poly2rbox": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "y5obb_gaussian_label": (c_int, [c_void_p, c_void_p, c_int64, c_int, ctypes.c_double, c_void_p]),
     "y5obb_bn_scratch_floats": (c_int64, [c_int]),
@@ -99,6 +100,8 @@ PROTOTYPES = {
     "y5obb_sppf_pool": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_scene_tiles_s2d_u8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                          c_void_p]),
+    "y5obb_letterbox_s2d_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int,
+                                       c_void_p]),
     "y5obb_scene_merge_workspace_bytes": (c_size_t, [c_int64, c_int, c_int, c_void_p]),
     "y5obb_scene_merge_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_float, c_float, ctypes.c_double,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

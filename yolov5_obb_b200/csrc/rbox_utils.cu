@@ -2,6 +2,7 @@
 //   y5obb_rbox2poly_f32      utils/rboxs_utils.py:106-126  (torch branch of rbox2poly)
 //   y5obb_poly2hbb_f32       utils/rboxs_utils.py:147-165  (torch branch of poly2hbb)
 //   y5obb_scale_polys_f32    utils/general.py:636-650      (scale_polys, in place)
+//   y5obb_scale_polys_batched_f32  both of the above for a batch's packed NMS rows, one (pad, gain) per image
 //   y5obb_gaussian_label     utils/rboxs_utils.py:9-26     (gaussian_label_cpu: 180-bin CSL row)
 // Each arithmetic step is a separately rounded fp32 op (no FMA contraction), like the chain of ATen
 // elementwise kernels it replaces; the CSL row is evaluated in fp64 like the numpy original.
@@ -36,6 +37,24 @@ __global__ void k_scale_polys(float* __restrict__ p, int64_t n, float padx, floa
   if (i >= n * 8) return;
   const float pad = (i & 1) ? pady : padx;
   p[i] = __fdiv_rn(__fsub_rn(p[i], pad), gain);
+}
+
+__global__ void k_scale_polys_batched(const float* __restrict__ rows7, const int64_t* __restrict__ counts,
+                                      const float* __restrict__ pg, int B, int max_det, float* __restrict__ polys) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)B * max_det) return;
+  const int b = (int)(i / max_det);
+  float poly[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (i - (int64_t)b * max_det < counts[b]) {
+    const float* r = rows7 + i * 7;
+    geom::rbox2poly_f32(r[0], r[1], r[2], r[3], r[4], poly);
+    const float gain = pg[3 * b + 2];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) poly[k] = __fdiv_rn(__fsub_rn(poly[k], pg[3 * b + (k & 1)]), gain);
+  }
+  float4* o = reinterpret_cast<float4*>(polys + i * 8);
+  o[0] = make_float4(poly[0], poly[1], poly[2], poly[3]);
+  o[1] = make_float4(poly[4], poly[5], poly[6], poly[7]);
 }
 
 __global__ void k_gaussian_label(const double* __restrict__ angle, float* __restrict__ out, int64_t n, int nc, double sig) {
@@ -81,6 +100,18 @@ int y5obb_scale_polys_f32(float* polys8, int64_t n, float pad_x, float pad_y, fl
   if (n == 0) return Y5OBB_OK;
   if (!polys8) return Y5OBB_EINVAL;
   k_scale_polys<<<(unsigned)((n * 8 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(polys8, n, pad_x, pad_y, gain);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+int y5obb_scale_polys_batched_f32(const float* rows7, const int64_t* counts, const float* pad_gain3, int B, int max_det,
+                                  float* polys8, void* stream) {
+  if (B < 0 || max_det < 0) return Y5OBB_EINVAL;
+  if (B == 0 || max_det == 0) return Y5OBB_OK;
+  if (!rows7 || !counts || !pad_gain3 || !polys8 || (reinterpret_cast<uintptr_t>(polys8) & 15)) return Y5OBB_EINVAL;
+  const int64_t n = (int64_t)B * max_det;
+  k_scale_polys_batched<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rows7, counts, pad_gain3, B, max_det,
+                                                                                    polys8);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
 }

@@ -226,7 +226,11 @@ class Validator:
     late, while the next batch computes, and the batch is then re-run with the blocking NMS from its device copy.
     compute_loss (a loss.ComputeLoss, train.py:364-373): the validation loss of val.py:198-199 is added per batch from the
     plan's Detect inputs (ComputeLoss.head_items) into a device fp32 sum, and `results` becomes val.py:333's
-    (mp, mr, map50, map, box, obj, cls, theta) with the loss sum divided by the number of batches."""
+    (mp, mr, map50, map, box, obj, cls, theta) with the loss sum divided by the number of batches.
+    Raw form: `im` may be the list of the batch's decoded source images (uint8 [h0, w0, 3] BGR arrays of any sizes) instead
+    of the letterboxed tensor.  `shapes` then says where each one lands (letterbox.place_rect(...).shapes, the rect loader's
+    entry); csrc/letterbox.cu resamples them as load_image_label + letterbox do and writes the plan's stem input, and
+    everything after the forward is the same.  targets stay in network-input pixels (Placement.map_labels)."""
 
     def __init__(self, model, conf_thres: float = 0.01, iou_thres: float = 0.4, max_det: int = 1500, iouv=None,
                  augment: bool = False, compute_loss=None):
@@ -246,6 +250,42 @@ class Validator:
         iouv = torch.linspace(0.5, 0.95, 10) if iouv is None else iouv
         self.iouv = iouv.detach().float().to(self.device)
         self.reruns = 0
+        self._raw_host, self._raw_ev, self._raw_n = [None, None], [None, None], 0   # pinned buffers of the raw form
+
+    def _upload_raw(self, images, shapes):
+        """The batch's source images, packed and uploaded with one copy -> (device buffer, letterbox.PackedBatch)."""
+        from . import letterbox as lb
+        if self.augment:
+            raise RuntimeError("test-time augmentation reads the letterboxed tensor: pass `im` as a tensor with augment=True")
+        if len(images) != len(shapes):
+            raise RuntimeError(f"{len(images)} images but {len(shapes)} shapes entries")
+        placed = [lb.place_from_shapes(s) for s in shapes]
+        hw = {p[1] for p in placed}
+        if len(hw) != 1:
+            raise RuntimeError(f"the shapes entries of one batch describe different letterboxed sizes: {sorted(hw)}")
+        (Hp, Wp), = hw
+        k = self._raw_n % 2
+        self._raw_n += 1
+        if self._raw_ev[k] is not None:
+            self._raw_ev[k].synchronize()   # the upload that last read this pinned buffer
+        batch = lb.pack_batch([lb.as_image(im) for im in images], [p[0] for p in placed], Hp, Wp, self._raw_host[k])
+        self._raw_host[k] = batch.host
+        buf = batch.host[:batch.nbytes].to(self.device, non_blocking=True)
+        self._raw_ev[k] = torch.cuda.Event()
+        self._raw_ev[k].record()
+        return buf, batch
+
+    def _records(self, x):
+        """detect_records for either form of a batch -> (DetectRecords, the plan's input shape)."""
+        if isinstance(x, torch.Tensor):
+            return self.model.detect_records(x, augment=self.augment), tuple(x.shape)
+        from . import letterbox as lb
+        from .general import DetectRecords
+        buf, batch = x
+        shape = (batch.B, 3, batch.Hp, batch.Wp)
+        eng = self.model.records_plan(shape, self.device)
+        lb.letterbox_s2d(buf, batch, eng.x_s2d, 1)
+        return DetectRecords(eng.forward_s2d(), eng.nc), shape
 
     def __call__(self, batches) -> ValMetrics:
         stats = ValStats(self.model.model[-1].nc, self.iouv.numel(), self.device)
@@ -267,11 +307,12 @@ class Validator:
 
     def _submit(self, stats, im, targets, shapes):
         from .general import non_max_suppression_obb
-        x, t = _upload(im, self.device), _upload(targets.float(), self.device)
+        x = self._upload_raw(im, shapes) if isinstance(im, (list, tuple)) else _upload(im, self.device)
+        t = _upload(targets.float(), self.device)
         base = stats.seen
-        recs = self.model.detect_records(x, augment=self.augment)
+        recs, shape = self._records(x)
         if self.compute_loss is not None:   # val.py:198-199; the overflow re-run in _settle does not add it again
-            self._loss += self.compute_loss.head_items(self.model.records_plan(tuple(x.shape), x.device), t)[1]
+            self._loss += self.compute_loss.head_items(self.model.records_plan(shape, self.device), t)[1]
         dets, counts, cap = non_max_suppression_obb(recs, return_packed="async", **self.nms)
         correct, _, _ = match_batch(dets, counts, t, shapes, self.iouv, want_geometry=False)
         skip = stats.add(dets, counts, correct, t, nms_cap=cap)
@@ -288,7 +329,7 @@ class Validator:
         if int(host[0]) == 0:
             return
         self.reruns += 1
-        dets, rows = non_max_suppression_obb(self.model.detect_records(x, augment=self.augment), return_packed=True, **self.nms)
+        dets, rows = non_max_suppression_obb(self._records(x)[0], return_packed=True, **self.nms)
         counts = torch.tensor(rows, dtype=torch.int64).to(self.device)
         correct, _, _ = match_batch(dets, counts, t, shapes, self.iouv, want_geometry=False)
         stats.add(dets, counts, correct, t, image_base=base)
