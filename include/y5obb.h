@@ -207,13 +207,14 @@ int y5obb_sppf_pool(void* buf, int64_t pix_stride, int B, int H, int W, int C, v
  * (loss.py:185-192).  backward writes dLoss/dp[i] * grad_loss[0] into grad[i] (dense, same shape as p[i]); it
  * must be given the workspace its forward filled.  Duplicate (b,a,gj,gi) cells: the highest source row wins
  * tobj, as sequential CPU index assignment does (loss.py:159). */
+#define Y5OBB_LOSS_MAX_LEVELS 4    /* P3-P5 (yolov5{n,s,m,l,x}) and P3-P6 (models/hub/yolov5{n,s,m,l,x}6); nl <= this */
 typedef struct {
-  const float* p[3];
-  float* grad[3];            /* backward only */
-  int H[3], W[3];
-  float stride[3];
-  float anchors[18];         /* Detect.anchors: [nl][na][2] in grid units */
-  float balance[3];          /* {4.0, 1.0, 0.4} (loss.py:114) */
+  const float* p[Y5OBB_LOSS_MAX_LEVELS];
+  float* grad[Y5OBB_LOSS_MAX_LEVELS];      /* backward only */
+  int H[Y5OBB_LOSS_MAX_LEVELS], W[Y5OBB_LOSS_MAX_LEVELS];
+  float stride[Y5OBB_LOSS_MAX_LEVELS];
+  float anchors[Y5OBB_LOSS_MAX_LEVELS * 3 * 2];  /* Detect.anchors: [nl][na][2] in grid units, na <= 3 */
+  float balance[Y5OBB_LOSS_MAX_LEVELS];    /* {4.0, 1.0, 0.4}; four levels {4.0, 1.0, 0.25, 0.06} (loss.py:114) */
   int nl, B, na, no, nc;
   const float* targets;
   int nt, tcols;
@@ -239,11 +240,12 @@ int y5obb_loss_backward(const y5obb_loss_desc* desc, const float* grad_loss, voi
  * elements, or feat / w is not 16-byte aligned.  The workspace holds the obj logits (4 bytes per cell) and
  * nl * 5 * na * nt rows of no floats besides y5obb_loss_forward's own. */
 typedef struct {
-  const void* feat[3];                   /* bf16 NHWC Detect input of level i (Detect.f[i]'s output) */
-  int64_t pix_stride[3], row_stride[3], img_stride[3];  /* element strides of pixels, rows and images */
-  int H[3], W[3], C[3];                  /* feature shape; C % 8 == 0 */
-  const void* w[3];                      /* bf16 [na * no, C]: Detect.m[i].weight */
-  const float* bias[3];                  /* fp32 [na * no]:    Detect.m[i].bias */
+  const void* feat[Y5OBB_LOSS_MAX_LEVELS];   /* bf16 NHWC Detect input of level i (Detect.f[i]'s output) */
+  int64_t pix_stride[Y5OBB_LOSS_MAX_LEVELS], row_stride[Y5OBB_LOSS_MAX_LEVELS],
+      img_stride[Y5OBB_LOSS_MAX_LEVELS];     /* element strides of pixels, rows and images */
+  int H[Y5OBB_LOSS_MAX_LEVELS], W[Y5OBB_LOSS_MAX_LEVELS], C[Y5OBB_LOSS_MAX_LEVELS];  /* feature shape; C % 8 == 0 */
+  const void* w[Y5OBB_LOSS_MAX_LEVELS];      /* bf16 [na * no, C]: Detect.m[i].weight */
+  const float* bias[Y5OBB_LOSS_MAX_LEVELS];  /* fp32 [na * no]:    Detect.m[i].bias */
 } y5obb_loss_head;
 
 size_t y5obb_loss_head_workspace_bytes(const y5obb_loss_desc* desc, const y5obb_loss_head* head);

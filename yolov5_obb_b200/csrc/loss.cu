@@ -35,15 +35,16 @@ namespace {
 
 constexpr int NOFF = 5;
 constexpr int OBJ_THREADS = 256;
+constexpr int NL = Y5OBB_LOSS_MAX_LEVELS;
 
 struct LossK {
-  const float* p[3];
-  float* grad[3];
-  int H[3], W[3];
-  long long cell_off[4];  // prefix of B*na*H*W per level
-  float stride[3];
-  float anchors[18];
-  float balance[3];
+  const float* p[NL];
+  float* grad[NL];
+  int H[NL], W[NL];
+  long long cell_off[NL + 1];  // prefix of B*na*H*W per level
+  float stride[NL];
+  float anchors[NL * 3 * 2];
+  float balance[NL];
   int nl, B, na, no, nc;
   const float* targets;
   int nt, tcols;
@@ -59,8 +60,8 @@ struct LossK {
   float* row_cls;     // sum over classes of BCE
   float* row_theta;   // sum over 180 bins of BCE
   double* obj_partial;  // [nl][obj_blocks]
-  int obj_blocks[3];
-  long long obj_block_off[4];
+  int obj_blocks[NL];
+  long long obj_block_off[NL + 1];
   int ncand;          // nl * 5 * na * nt
   // Circular-Smooth-Label rows (utils/rboxs_utils.py:9-26): csl_mode 0 = 180 floats per target at column 7 (the reference's
   // [nt,187] layout), 1 = column 7 holds the row's rotation index int(90 - angle) (the caller evaluated the truncation in
@@ -70,9 +71,9 @@ struct LossK {
   // Where k_rows and k_obj read the logits.  A matched row's no logits start at
   // rows[lvl] + cell_local * row_cell_stride + rank * row_rank_stride; cell i's obj logit is obj[lvl][i * obj_stride + obj_col].
   // The materialised head gives (p, no, 0) and (p, no, 4); the Detect-input path gives its workspace buffers (0, no) and (1, 0).
-  const float* rows[3];
+  const float* rows[NL];
   long long row_cell_stride, row_rank_stride;
-  const float* obj[3];
+  const float* obj[NL];
   long long obj_stride;
   int obj_col;
   void* scan_tmp;
@@ -335,8 +336,10 @@ struct HeadLevel {
   const float* bias;          // [na * no]
 };
 struct HeadK {
-  HeadLevel lv[3];
+  HeadLevel lv[NL];
 };
+// k_head_rows takes both blocks as its launch parameters (4 KB at most on sm_90)
+static_assert(sizeof(LossK) + sizeof(HeadK) <= 4096, "loss kernel parameters exceed the 4 KB launch-parameter limit");
 
 // 8 bf16 products of two 16-byte vectors, accumulated in order into acc
 __device__ __forceinline__ float dot8(const uint4& x, const uint4& y, float acc) {
@@ -521,7 +524,7 @@ __global__ void k_bwd_rows(LossK L, const float* __restrict__ gloss) {
 }
 
 int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* need, bool head = false) {
-  if (!d || d->nl < 1 || d->nl > 3 || d->B < 1 || d->na < 1 || d->na > 3 || d->nt < 0) return Y5OBB_EINVAL;
+  if (!d || d->nl < 1 || d->nl > NL || d->B < 1 || d->na < 1 || d->na > 3 || d->nt < 0) return Y5OBB_EINVAL;
   if (d->no != d->nc + 5 + 180 || d->no % 4) return Y5OBB_EINVAL;
   if (d->tcols != 7 && d->tcols != 8 && d->tcols < 7 + 180) return Y5OBB_EINVAL;
   memset(&L, 0, sizeof(L));
@@ -572,7 +575,7 @@ int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* 
   L.row_rank_stride = 0;
   L.obj_col = 4;
   L.obj_block_off[d->nl] = blocks;
-  for (int i = 0; i < 18; ++i) L.anchors[i] = d->anchors[i];
+  for (int i = 0; i < NL * 3 * 2; ++i) L.anchors[i] = d->anchors[i];
   L.ncand = d->nl * NOFF * d->na * d->nt;
   const int nc1 = L.ncand > 0 ? L.ncand : 1;
   Carver c(ws);
@@ -651,7 +654,7 @@ int forward(LossK& L, const HeadK* hk, float* loss1, float* items4, cudaStream_t
 
 // Checks the Detect inputs and gives the loss description they imply: H / W from the features, no materialised logits.
 int head_desc(const y5obb_loss_desc* d, const y5obb_loss_head* h, y5obb_loss_desc* dd, HeadK* hk) {
-  if (!d || !h || d->nl < 1 || d->nl > 3 || d->na < 1 || d->na > 3 || d->no < 1) return Y5OBB_EINVAL;
+  if (!d || !h || d->nl < 1 || d->nl > NL || d->na < 1 || d->na > 3 || d->no < 1) return Y5OBB_EINVAL;
   *dd = *d;
   memset(hk, 0, sizeof(*hk));
   for (int i = 0; i < d->nl; ++i) {

@@ -14,12 +14,14 @@ import torch
 
 from . import _lib
 
+MAX_LEVELS = 4  # Y5OBB_LOSS_MAX_LEVELS (include/y5obb.h): the P3-P6 Detect of models/hub/yolov5*6.yaml
+
 
 class LossDesc(ctypes.Structure):
     """Mirror of y5obb_loss_desc (include/y5obb.h)."""
     _fields_ = [
-        ("p", c_void_p * 3), ("grad", c_void_p * 3), ("H", c_int * 3), ("W", c_int * 3), ("stride", c_float * 3),
-        ("anchors", c_float * 18), ("balance", c_float * 3),
+        ("p", c_void_p * MAX_LEVELS), ("grad", c_void_p * MAX_LEVELS), ("H", c_int * MAX_LEVELS), ("W", c_int * MAX_LEVELS),
+        ("stride", c_float * MAX_LEVELS), ("anchors", c_float * (MAX_LEVELS * 3 * 2)), ("balance", c_float * MAX_LEVELS),
         ("nl", c_int), ("B", c_int), ("na", c_int), ("no", c_int), ("nc", c_int),
         ("targets", c_void_p), ("nt", c_int), ("tcols", c_int),
         ("anchor_t", c_float), ("cp", c_float), ("cn", c_float),
@@ -31,8 +33,9 @@ class LossDesc(ctypes.Structure):
 class LossHead(ctypes.Structure):
     """Mirror of y5obb_loss_head (include/y5obb.h)."""
     _fields_ = [
-        ("feat", c_void_p * 3), ("pix_stride", c_int64 * 3), ("row_stride", c_int64 * 3), ("img_stride", c_int64 * 3),
-        ("H", c_int * 3), ("W", c_int * 3), ("C", c_int * 3), ("w", c_void_p * 3), ("bias", c_void_p * 3),
+        ("feat", c_void_p * MAX_LEVELS), ("pix_stride", c_int64 * MAX_LEVELS), ("row_stride", c_int64 * MAX_LEVELS),
+        ("img_stride", c_int64 * MAX_LEVELS), ("H", c_int * MAX_LEVELS), ("W", c_int * MAX_LEVELS), ("C", c_int * MAX_LEVELS),
+        ("w", c_void_p * MAX_LEVELS), ("bias", c_void_p * MAX_LEVELS),
     ]
 
 
@@ -95,8 +98,10 @@ class ComputeLoss:
         self.gr, self.hyp, self.autobalance = 1.0, h, autobalance
         for k in "na", "nc", "nl", "anchors":
             setattr(self, k, getattr(det, k))
-        if self.nl != 3 or self.na > 3:
-            raise RuntimeError("only the 3-level / 3-anchor Detect of yolov5{n,s,m,l,x}.yaml is built")
+        if self.nl not in (3, MAX_LEVELS) or self.na > 3:
+            raise RuntimeError(f"the loss takes the 3-level Detect of yolov5{{n,s,m,l,x}}.yaml or the {MAX_LEVELS}-level one of "
+                               f"models/hub/yolov5{{n,s,m,l,x}}6.yaml, with at most 3 anchors per level; this one has "
+                               f"nl={self.nl}, na={self.na}")
         self._anchors_host = [float(v) for v in self.anchors.detach().float().cpu().flatten().tolist()]
         self._stride_host = [float(s) for s in self.stride]
 

@@ -189,13 +189,14 @@ class DetectPipeline:
         return [hout[b, :k].clone() for b, k in enumerate(c[:B])]
 
     # ------------------------------------------------------------------ decoded images of any size
-    def run_images(self, images, img_size: int = 1024, stride: int = 32, auto: bool = True, batch_size: int = 1,
+    def run_images(self, images, img_size: int = 1024, stride: Optional[int] = None, auto: bool = True, batch_size: int = 1,
                    pad: float = 0.0) -> Iterator[ImageDetections]:
         """images: uint8 [H, W, 3] BGR arrays (numpy or CPU tensors, as cv2.imread returns them) of any sizes.  Yields one
         ImageDetections per image, in input order.  Two modes, both the reference's:
         * auto=True, detect.py: each image is letterboxed on its own to the minimum rectangle (INTER_LINEAR, scale-up
-          allowed, 114 border up to a multiple of `stride`), one image per forward (batch_size must be 1), polygons scaled
-          back from the two shapes (detect.py:147).  `images` may be any iterable.
+          allowed, 114 border up to a multiple of `stride`, by default the model's largest stride as in detect.py:81-82),
+          one image per forward (batch_size must be 1), polygons scaled back from the two shapes (detect.py:147).
+          `images` may be any iterable.
         * auto=False, val.py's rect loader: `images` is a sequence; the images are sorted by aspect ratio and grouped
           (rect_batch_shapes with `pad`), each resized so that its longer side is img_size (INTER_AREA when shrinking) and
           letterboxed without scale-up into its batch's shape, polygons scaled back with the loader's `shapes` (val.py:232).
@@ -203,8 +204,8 @@ class DetectPipeline:
         img_size / stride distinct auto=True shapes (32 at 1024), each planned on first use."""
         if not self.fused:
             raise RuntimeError("run_images runs the fused records plan (fused_detect=True)")
-        img_size, stride, batch_size = int(img_size), int(stride), int(batch_size)
         smax = int(max(self.model.stride))
+        img_size, stride, batch_size = int(img_size), smax if stride is None else int(stride), int(batch_size)
         if stride < 1 or stride % smax or img_size < stride or img_size % stride:
             raise RuntimeError(f"img_size ({img_size}) must be a multiple of stride ({stride}), and stride a multiple of the "
                                f"model's largest stride ({smax})")

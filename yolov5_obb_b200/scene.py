@@ -43,13 +43,16 @@ def split_origins(height: int, width: int, subsize: int = 1024, gap: int = 200) 
     return out
 
 
-def tile_geometry(subsize: int = 1024, pad: float = 0.5) -> Tuple[int, int, float]:
-    """(size, border, pad_xy): the inference size of a tile as val.py's rect batching makes it, ceil(subsize / 32 + pad) * 32
-    (utils/datasets.py:492), the letterbox border on the top / left, int(round(d - 0.1)) with d = (size - subsize) / 2, and d
+def tile_geometry(subsize: int = 1024, pad: float = 0.5, stride: int = 32) -> Tuple[int, int, float]:
+    """(size, border, pad_xy): the inference size of a tile as val.py's rect batching makes it with the model's largest
+    stride, ceil(subsize / stride + pad) * stride (utils/datasets.py:492; 1056 for a P5 model, 1088 for a P6 model at subsize
+    1024 and pad 0.5), the letterbox border on the top / left, int(round(d - 0.1)) with d = (size - subsize) / 2, and d
     itself, which scale_polys subtracts (utils/augmentations.py:92-128 with auto=False, scaleup=False)."""
     if pad < 0:
         raise RuntimeError(f"pad must be >= 0, got {pad}")
-    size = int(math.ceil(subsize / 32 + pad)) * 32
+    if stride < 1:
+        raise RuntimeError(f"stride must be >= 1, got {stride}")
+    size = int(math.ceil(subsize / stride + pad)) * stride
     d = (size - subsize) / 2
     return size, int(round(d - 0.1)), d
 
@@ -128,8 +131,9 @@ class SceneDetector:
     """Scene (uint8 [H, W, 3] BGR on a CUDA device, as cv2.imread decodes it) -> SceneDetections, as the reference's
     ImgSplit (rate 1) -> val.py --conf conf_thres --iou iou_thres --save-json -> TestJson2VocClassTxt -> ResultMerge chain
     computes them.  Tiles run in batches of batch_size through one records plan; the last batch runs the full plan and the
-    detections of its padding tiles are ignored.  pad=0.5 is val.py's rect-batching pad (1056^2 tiles for subsize 1024),
-    pad=0.0 the unpadded tile of detect.py / --task speed."""
+    detections of its padding tiles are ignored.  pad=0.5 is val.py's rect-batching pad (1056^2 tiles for subsize 1024,
+    1088^2 for a stride-64 P6 model: the size is rounded to the model's largest stride), pad=0.0 the unpadded tile of detect.py /
+    --task speed.  The model is one of the two families the engine plans: P5 (strides 8, 16, 32) or P6 (8, 16, 32, 64)."""
 
     def __init__(self, model, batch_size: int = 16, subsize: int = 1024, gap: int = 200, conf_thres: float = 0.01,
                  iou_thres: float = 0.4, max_det: int = 1500, merge_thresh: float = 0.2, pad: float = 0.5):
@@ -137,10 +141,11 @@ class SceneDetector:
             raise RuntimeError(f"gap ({gap}) must be in [0, subsize) (subsize {subsize})")
         if batch_size < 1 or max_det < 1:
             raise RuntimeError("batch_size and max_det must be >= 1")
-        self.size, self.border, self.pad_xy = tile_geometry(subsize, pad)
-        smax = int(max(model.stride))
-        if self.size % smax:
-            raise RuntimeError(f"tile inference size {self.size} is not a multiple of the model stride {smax}")
+        strides = [float(v) for v in model.stride]
+        if strides not in ([8.0, 16.0, 32.0], [8.0, 16.0, 32.0, 64.0]):
+            raise RuntimeError(f"the model's Detect strides {strides} are neither the P5 layout (8, 16, 32) of yolov5*.yaml nor "
+                               "the P6 layout (8, 16, 32, 64) of models/hub/yolov5*6.yaml")
+        self.size, self.border, self.pad_xy = tile_geometry(subsize, pad, int(strides[-1]))
         self.model, self.B, self.subsize, self.gap = model, int(batch_size), int(subsize), int(gap)
         self.conf_thres, self.iou_thres, self.max_det, self.merge_thresh = conf_thres, iou_thres, int(max_det), merge_thresh
         self._status_host = None

@@ -16,10 +16,12 @@ import torch
 import torch.nn as nn
 
 # ---------------------------------------------------------------------------------------------
-# configuration (values of models/yolov5{n,s,m,l,x}.yaml, generated rather than stored)
+# configuration (values of models/yolov5{n,s,m,l,x}.yaml and models/hub/yolov5{n,s,m,l,x}6.yaml, generated rather than stored)
 # ---------------------------------------------------------------------------------------------
 _SCALES = {"n": (0.33, 0.25), "s": (0.33, 0.50), "m": (0.67, 0.75), "l": (1.0, 1.0), "x": (1.33, 1.25)}
 _ANCHORS = [[10, 13, 16, 30, 33, 23], [30, 61, 62, 45, 59, 119], [116, 90, 156, 198, 373, 326]]  # P3/8, P4/16, P5/32
+_ANCHORS_P6 = [[19, 27, 44, 40, 38, 94], [96, 68, 86, 152, 180, 137], [140, 301, 303, 264, 238, 542],
+               [436, 615, 739, 380, 925, 792]]  # P3/8, P4/16, P5/32, P6/64
 
 
 def yolov5_cfg(size: str = "s", nc: int = 80) -> dict:
@@ -37,6 +39,24 @@ def yolov5_cfg(size: str = "s", nc: int = 80) -> dict:
         head += [[-1, 1, "Conv", [width, 3, 2]], [[-1, skip], 1, "Concat", [1]], [-1, 3, "C3", [2 * width, False]]]
     head += [[[17, 20, 23], 1, "Detect", ["nc", "anchors"]]]          # 24
     return dict(nc=nc, depth_multiple=gd, width_multiple=gw, anchors=deepcopy(_ANCHORS), backbone=backbone, head=head)
+
+
+def yolov5_p6_cfg(size: str = "s", nc: int = 80) -> dict:
+    """The four-level layout of models/hub/yolov5s6.yaml:13-58 (one more stride-2 stage to P6/64, a 768-wide P5 stage, a
+    fourth Detect level) for a given scale letter; the multipliers are those of the P5 family."""
+    gd, gw = _SCALES[size]
+    backbone = [[-1, 1, "Conv", [64, 6, 2, 2]]]                                      # 0  P1/2
+    for width, depth in ((128, 3), (256, 6), (512, 9), (768, 3), (1024, 3)):         # 1-10: stride-2 conv + C3 per stage
+        backbone += [[-1, 1, "Conv", [width, 3, 2]], [-1, depth, "C3", [width]]]
+    backbone += [[-1, 1, "SPPF", [1024, 5]]]                                          # 11
+    head = []
+    for width, skip in ((768, 8), (512, 6), (256, 4)):                                # top-down: 12-23
+        head += [[-1, 1, "Conv", [width, 1, 1]], [-1, 1, "nn.Upsample", [None, 2, "nearest"]],
+                 [[-1, skip], 1, "Concat", [1]], [-1, 3, "C3", [width, False]]]
+    for width, skip, out in ((256, 20, 512), (512, 16, 768), (768, 12, 1024)):         # bottom-up: 24-32
+        head += [[-1, 1, "Conv", [width, 3, 2]], [[-1, skip], 1, "Concat", [1]], [-1, 3, "C3", [out, False]]]
+    head += [[[23, 26, 29, 32], 1, "Detect", ["nc", "anchors"]]]                      # 33
+    return dict(nc=nc, depth_multiple=gd, width_multiple=gw, anchors=deepcopy(_ANCHORS_P6), backbone=backbone, head=head)
 
 
 def make_divisible(x, divisor):
@@ -193,7 +213,7 @@ class _TrainFn(torch.autograd.Function):
 
 class Model(nn.Module):
     """Drop-in for models/yolo.py:95 Model: Model(cfg, ch=3, nc=None, anchors=None); forward(x[B,3,H,W] in [0,1])
-    -> eval: (pred[B, sum(3*H_i*W_i), nc+185] fp32, None); train: list of 3 [B,3,H_i,W_i,nc+185] logits."""
+    -> eval: (pred[B, sum(3*H_i*W_i), nc+185] fp32, None); train: list of nl (3, or 4 for P6) [B,3,H_i,W_i,nc+185] logits."""
 
     def __init__(self, cfg="yolov5s.yaml", ch=3, nc=None, anchors=None):
         super().__init__()
@@ -206,12 +226,15 @@ class Model(nn.Module):
                 self.yaml_file = p.name
                 with open(p, encoding="ascii", errors="ignore") as f:
                     self.yaml = yaml.safe_load(f)
-            else:  # "yolov5s.yaml" / "yolov5s" / "s"
+            else:  # "yolov5s.yaml" / "yolov5s" / "s", "yolov5s6.yaml" / "yolov5s6" / "s6"
                 key = p.stem.replace("yolov5", "")
-                if key not in _SCALES:
+                if key in _SCALES:
+                    self.yaml = yolov5_cfg(key)
+                elif key[-1:] == "6" and key[:-1] in _SCALES:
+                    self.yaml = yolov5_p6_cfg(key[:-1])
+                else:
                     raise FileNotFoundError(cfg)
                 self.yaml_file = f"yolov5{key}.yaml"
-                self.yaml = yolov5_cfg(key)
         ch = self.yaml["ch"] = self.yaml.get("ch", ch)
         if nc and nc != self.yaml["nc"]:
             self.yaml["nc"] = nc
@@ -311,7 +334,7 @@ class Model(nn.Module):
         return eng.forward(x), None
 
     def forward_train(self, x, size=None):
-        """Training-mode forward (what forward(x) runs in train()): list of 3 raw [B, 3, H_i, W_i, nc+185] logits.
+        """Training-mode forward (what forward(x) runs in train()): list of nl raw [B, 3, H_i, W_i, nc+185] logits.
         size=(h, w): train.py's --multi-scale resize, `F.interpolate(x, size=size, mode='bilinear', align_corners=False)`,
         runs as the plan's first launch (the plan takes the un-resized x; plans are keyed by input shape and size).
         With a reserved arena (reserve_train_arena) the returned tensors live in it: the next training forward of ANY
