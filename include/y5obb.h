@@ -332,15 +332,11 @@ void y5obb_wgrad_destroy(y5obb_wgrad_t* w);
 
 /* backward helpers of the training graph (NHWC bf16 gradients):
  *   upsample2x_bwd   nn.Upsample(2x nearest) backward: gdst (+)= 2x2 block sums of gsrc
- *   zero_stuff2x     dst[b,2h,2w,:] = src[b,h,w,:] into a pre-zeroed buffer: the dgrad of a stride-2 conv then is a
- *                    stride-1 conv over it with flipped, transposed weights
  *   maxpool5_bwd     one MaxPool2d(5,1,2) backward step of SPPF (models/common.py:190-196) into an fp32 buffer
  *   add_f32_to_bf16  bf16 slice (+)= fp32 dense buffer
  *   detect_grad_pack loss gradient fp32 [B,na,H,W,no] -> bf16 NHWC [B,H,W,na*bn] (the Detect conv's dz) */
 int y5obb_upsample2x_bwd(const void* gsrc, int64_t src_pix_stride, void* gdst, int64_t dst_pix_stride, int64_t npix_dst,
                          int C, int W_dst, int accumulate, void* stream);
-int y5obb_zero_stuff2x(const void* src, int64_t src_pix_stride, void* dst, int64_t dst_pix_stride, int64_t npix_src, int C,
-                       int W_src, void* stream);
 int y5obb_maxpool5_bwd(const void* x_in, int64_t in_pix_stride, const float* gout_f32, const void* gout_bf16,
                        int64_t gout_pix_stride, float* gin_f32, int B, int H, int W, int C, void* stream);
 int y5obb_add_f32_to_bf16(const float* src, void* dst, int64_t dst_pix_stride, int64_t npix, int C, int accumulate,

@@ -212,19 +212,18 @@ def test_wgmma_accumulation_is_exact_below_2p24():
 
 # ---------------------------------------------------------------------------------------------------------------------
 PLANS = [
-    pytest.param("s", 16, 1024, 1024, "forward", None, id="yolov5s-b16-1024-forward"),
-    pytest.param("s", 16, 1024, 1024, "records", None, id="yolov5s-b16-1024-records"),
-    pytest.param("m", 16, 1024, 1024, "forward", None, id="yolov5m-b16-1024-forward"),
-    pytest.param("m", 8, 1024, 1024, "train", None, id="yolov5m-b8-1024-train"),
-    pytest.param("n", 2, 96, 160, "train", None, id="yolov5n-b2-96x160-train"),
-    pytest.param("n", 2, 96, 160, "forward", None, id="yolov5n-b2-96x160-forward"),
-    pytest.param("n", 2, 96, 160, "records", None, id="yolov5n-b2-96x160-records"),
-    pytest.param("n", 2, 96, 160, "train", "zero-stuffed", id="yolov5n-b2-96x160-train-zero-stuffed-dgrad"),
+    pytest.param("s", 16, 1024, 1024, "forward", id="yolov5s-b16-1024-forward"),
+    pytest.param("s", 16, 1024, 1024, "records", id="yolov5s-b16-1024-records"),
+    pytest.param("m", 16, 1024, 1024, "forward", id="yolov5m-b16-1024-forward"),
+    pytest.param("m", 8, 1024, 1024, "train", id="yolov5m-b8-1024-train"),
+    pytest.param("n", 2, 96, 160, "train", id="yolov5n-b2-96x160-train"),
+    pytest.param("n", 2, 96, 160, "forward", id="yolov5n-b2-96x160-forward"),
+    pytest.param("n", 2, 96, 160, "records", id="yolov5n-b2-96x160-records"),
 ]
 
 
-@pytest.mark.parametrize("size,B,H,W,kind,dgrad_s2", PLANS)
-def test_every_launch_matches_its_descriptor(size, B, H, W, kind, dgrad_s2, monkeypatch):
+@pytest.mark.parametrize("size,B,H,W,kind", PLANS)
+def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
     """Every launch against its own descriptor (tests/convref.py).  Bitwise: every act=False conv (train forward, every dgrad
     form), raw Detect rows, every wgrad (split-K over the whole pixel axis, the stem's window view, Detect's padded
     channel groups), out2x against the repeated output.  Theta index of records: the first maximum, exactly.  Within a bound
@@ -235,8 +234,6 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind, dgrad_s2, monk
       * decoded Detect rows and records: the sigmoid 0.5 tanh.approx(0.5 x) + 0.5 errs by at most half of tanh's error (+ one
         fp32 rounding), propagated through the decode (x 2 stride for xy, x 8 anchor for wh) plus the fp32 roundings of the
         decode arithmetic."""
-    if dgrad_s2:
-        monkeypatch.setenv("Y5OBB_DGRAD_S2", dgrad_s2)
     torch.manual_seed(2)
     m = build_mirror(size, nc=15, seed=0)
     convs, wgrads = [], []
@@ -244,7 +241,7 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind, dgrad_s2, monk
         m = m.train().to(DEV)
         eng = TrainEngine(m, B, H, W, DEV)
         plan = BackwardPlan(eng)
-        convs = [lay.conv for lay in eng.layers if not isinstance(lay, tuple)] + list(eng.det_convs)
+        convs = [lay.conv for lay in eng.conv_layers] + list(eng.det_convs)
         bwd = []
         for part in plan.det_parts + plan.conv_parts:
             bwd += part.get("dgrad_ops", [])
@@ -252,7 +249,7 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind, dgrad_s2, monk
         # the parts list every conv / wgrad object the backward plan keeps
         assert {id(o) for o in plan.keep if isinstance(o, (ConvOp, Wgrad))} == {id(o) for o in bwd + wgrads}
         s2 = [len(p["dgrad_ops"]) for p in plan.conv_parts if "dgrad_ops" in p and p["lay"].mod.conv.stride[0] == 2]
-        assert s2 and all(n == (1 if dgrad_s2 else 4) for n in s2), s2
+        assert s2 and all(n == 4 for n in s2), s2
         convs += bwd
     else:
         eng = InferenceEngine(m, B, H, W, DEV, compact_detect=kind == "records")
@@ -262,7 +259,7 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind, dgrad_s2, monk
         check_conv(op, st, f"conv {i}")
     for i, wg in enumerate(wgrads):
         check_wgrad(wg, st, f"wgrad {i}")
-    print(f"\n{size} b{B} {H}x{W} {kind}{' ' + dgrad_s2 if dgrad_s2 else ''}: {st['conv']} conv and {st['wgrad']} wgrad "
+    print(f"\n{size} b{B} {H}x{W} {kind}: {st['conv']} conv and {st['wgrad']} wgrad "
           f"launches checked; {st['bitwise']} bitwise, {st['tolerance']} within the epilogue bound "
           f"(worst {st['worst']:.3f} of it)" + (f"; theta ties in {st['ties']} of {st['rows']} records rows"
                                                    if kind == "records" else ""))

@@ -109,7 +109,7 @@ def test_schedule_is_bit_identical_to_one_cta(size, B, kind):
         m = m.train().to(DEV)
         eng = TrainEngine(m, B, 1024, 1024, DEV)
         plan = BackwardPlan(eng)
-        convs = [lay.conv for lay in eng.layers if not isinstance(lay, tuple)] + list(eng.det_convs)
+        convs = [lay.conv for lay in eng.conv_layers] + list(eng.det_convs)
         for part in plan.det_parts + plan.conv_parts:
             convs += part.get("dgrad_ops", [])
     else:

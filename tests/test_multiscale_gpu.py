@@ -155,7 +155,7 @@ def test_every_launch_of_arena_plans_matches_its_descriptor():
         with torch.no_grad():
             eng.forward(x)                                       # the plan uses the arena after the larger one did
         plan = BackwardPlan(eng)
-        convs = [lay.conv for lay in eng.layers if not isinstance(lay, tuple)] + list(eng.det_convs)
+        convs = [lay.conv for lay in eng.conv_layers] + list(eng.det_convs)
         wgrads = []
         for part in plan.det_parts + plan.conv_parts:
             convs += part.get("dgrad_ops", [])

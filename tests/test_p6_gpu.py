@@ -413,6 +413,6 @@ def test_augment_loader_at_a_multiple_of_64():
 # ---- every conv / dgrad / wgrad launch, exact under integer operands -------------------------------------------------
 @pytest.mark.parametrize("size,B,H,W,kind", [("s6", 16, 1280, 1280, "forward"), ("s6", 8, 1024, 1024, "train")],
                          ids=["yolov5s6-b16-1280-forward", "yolov5s6-b8-1024-train"])
-def test_every_launch_matches_its_descriptor(size, B, H, W, kind, monkeypatch):
+def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
     _release_memory()
-    CE.test_every_launch_matches_its_descriptor(size, B, H, W, kind, None, monkeypatch)
+    CE.test_every_launch_matches_its_descriptor(size, B, H, W, kind)

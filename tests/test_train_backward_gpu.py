@@ -18,6 +18,8 @@ import torch.nn.functional as F
 
 from oracle import model_ref
 from tests.modelgen import build_mirror
+from yolov5_obb_b200.layout import sources
+from yolov5_obb_b200.train_engine import _PoolLayer
 import yolov5_obb_b200.yolo as Y
 
 pytestmark = pytest.mark.gpu
@@ -40,17 +42,14 @@ def _teacher_forced(md, ref_m, eng, x, G):
         gb = plan.gbuf[s.buf.data_ptr()]
         return gb[..., s.c_off:s.c_off + s.C].float().permute(0, 3, 1, 2).contiguous().cpu()
 
-    def src_of(i, f):
-        return i - 1 if f == -1 else f
-
     def resolve(j):
         m = mods[j]
         if j in real:
             return leaves[j]
         if isinstance(m, Y.Concat):
-            return torch.cat([resolve(src_of(j, f)) for f in m.f], 1)
+            return torch.cat([resolve(s) for s in sources(m)], 1)
         if isinstance(m, Y.Upsample):
-            return F.interpolate(resolve(src_of(j, m.f)), scale_factor=2, mode="nearest")
+            return F.interpolate(resolve(sources(m)[0]), scale_factor=2, mode="nearest")
         raise AssertionError(type(m))
 
     ref_m.zero_grad()
@@ -59,11 +58,11 @@ def _teacher_forced(md, ref_m, eng, x, G):
     with torch.enable_grad():
         for i, m in enumerate(mods):
             if i in real:
-                xin = x.bfloat16().float() if i == 0 else resolve(src_of(i, m.f))
+                xin = x.bfloat16().float() if i == 0 else resolve(sources(m)[0])
                 if isinstance(m, Y.SPPF):
                     # two teacher-forced pieces: cv1 | max-pools + cv2 on the device's own cv1 output (the arg-max
                     # of a max-pool is decided by the STORED bf16 values; recomputing them in fp32 would move maxima)
-                    cat4 = [l for l in eng.layers if isinstance(l, tuple)][0][1]
+                    cat4 = [l for l in eng.layers if isinstance(l, _PoolLayer)][0].cat4
                     c_ = m.cv1.conv.out_channels
                     y1 = cat4[..., :c_].float().permute(0, 3, 1, 2).contiguous().cpu().requires_grad_(True)
                     g_y1 = plan.gbuf[cat4.data_ptr()][..., :c_].float().permute(0, 3, 1, 2).contiguous().cpu()

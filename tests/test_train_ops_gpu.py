@@ -142,7 +142,7 @@ def test_wgrad_param_layout_and_padded_groups():
 def test_pack_plan_matches_host_packing():
     """One-launch device packing (csrc/pack_weights.cu) == conv.pack_weights on the host-side formulas, every kind."""
     from yolov5_obb_b200.conv import pack_weights, MODE_DETECT, tiling
-    from yolov5_obb_b200.train_engine import TrainEngine
+    from yolov5_obb_b200.layout import stem_weight
     from yolov5_obb_b200.train_ops import (PackPlan, PACK_FWD, PACK_DGRAD, PACK_STEM, PACK_DETECT, PACK_DETECT_DGRAD,
                                            PACK_DETECT_BIAS)
     g = torch.Generator().manual_seed(3)
@@ -158,7 +158,7 @@ def test_pack_plan_matches_host_packing():
         add(PACK_FWD, w, pack_weights(w, None)[0])
         add(PACK_DGRAD, w, pack_weights(w.permute(1, 0, 2, 3).flip(2, 3).contiguous(), None)[0])
     w = torch.randn(48, 3, 6, 6, generator=g).to(DEV)
-    add(PACK_STEM, w, pack_weights(TrainEngine._stem_weight(w), None)[0])
+    add(PACK_STEM, w, pack_weights(stem_weight(w), None)[0])
     na, no, cin = 3, 200, 192
     w = torch.randn(na * no, cin, 1, 1, generator=g).to(DEV)
     b = torch.randn(na * no, generator=g).to(DEV)

@@ -27,9 +27,9 @@ from tests import bnref
 from tests.bnref import U, gamma, stat_chain, ulp32
 from tests.modelgen import build_mirror
 from yolov5_obb_b200 import _lib
-from yolov5_obb_b200.engine import _is
+from yolov5_obb_b200.layout import _is, sources
 from yolov5_obb_b200.train_backward import BackwardPlan
-from yolov5_obb_b200.train_engine import TrainEngine
+from yolov5_obb_b200.train_engine import TrainEngine, _PoolLayer
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -389,22 +389,6 @@ def test_upsample2x_bwd(B, H, W, C, acc):
     note("upsample2x_bwd (bitwise)", 0.0)
 
 
-@pytest.mark.parametrize("B,H,W,C", [(2, 5, 7, 16), (1, 1, 1, 8), (1, 4, 6, 2056), (3, 3, 4, 96)])
-def test_zero_stuff2x(B, H, W, C):
-    g = torch.Generator(device=DEV).manual_seed(B * H + W + C)
-    sbuf, sv = slab((B, H, W), C, extra=16, c_off=8, fill=IN_SENT)
-    sv.copy_(torch.randn(B, H, W, C, device=DEV, generator=g).bfloat16())
-    dbuf, dv = slab((B, 2 * H, 2 * W), C, extra=16, c_off=16)
-    before = dbuf.clone()
-    assert lib().y5obb_zero_stuff2x(sv.data_ptr(), sbuf.shape[-1], dv.data_ptr(), dbuf.shape[-1], B * H * W, C, W, stream()) == 0
-    torch.cuda.synchronize()
-    assert torch.equal(bits(dv[:, 0::2, 0::2]), bits(sv)), "zero_stuff2x: even positions"
-    m = torch.zeros(dbuf.shape, dtype=torch.bool, device=DEV)
-    m[:, 0::2, 0::2, 16:16 + C] = True
-    unchanged(dbuf, before, m, "zero_stuff2x (odd positions and other channels)")
-    note("zero_stuff2x (bitwise)", 0.0)
-
-
 @pytest.mark.parametrize("npix,C,stride,c_off", [(37, 24, 40, 8), (5, 13, 16, 3), (4096, 96, 128, 16), (1, 8, 8, 0)])
 @pytest.mark.parametrize("acc", [0, 1])
 def test_add_f32_to_bf16(npix, C, stride, c_off, acc):
@@ -466,9 +450,8 @@ def test_maxpool5_bwd(B, H, W, C, form):
 
 
 # =========================================================================================================== 2. the plans
-PLANS = [pytest.param("m", 8, 1024, 1024, None, id="yolov5m-b8-1024"),
-         pytest.param("s", 2, 256, 320, None, id="yolov5s-b2-256x320"),
-         pytest.param("s", 2, 256, 320, "zero-stuffed", id="yolov5s-b2-256x320-zero-stuffed-dgrad")]
+PLANS = [pytest.param("m", 8, 1024, 1024, id="yolov5m-b8-1024"),
+         pytest.param("s", 2, 256, 320, id="yolov5s-b2-256x320")]
 
 
 class _Recorder:
@@ -500,8 +483,8 @@ def _randomise_bn(m, g):
                 mod.running_var.copy_(0.5 + torch.rand(C, device=DEV, generator=g))
 
 
-@pytest.mark.parametrize("size,B,H,W,dgrad_s2", PLANS[:2])
-def test_plan_forward_bn_launches(size, B, H, W, dgrad_s2):
+@pytest.mark.parametrize("size,B,H,W", PLANS)
+def test_plan_forward_bn_launches(size, B, H, W):
     """Every bn_batch_stats / bn_silu_apply pair of the train plan, issued with the arguments _forward_eager passes, on
     controlled z (|mean| / sigma cycling through 0, 3, 10) with every other element of the destination buffers a sentinel."""
     m, eng = _plan(size, B, H, W)
@@ -516,7 +499,7 @@ def test_plan_forward_bn_launches(size, B, H, W, dgrad_s2):
         eng._L = real
     stats = [a for n, a in rec.calls if n == "y5obb_bn_batch_stats"]
     apply = [a for n, a in rec.calls if n == "y5obb_bn_silu_apply"]
-    lays = [lay for lay in eng.layers if not isinstance(lay, tuple)]
+    lays = eng.conv_layers
     assert len(stats) == len(apply) == len(lays)
     L, st = lib(), stream()
     n_y2x = n_res = 0
@@ -573,13 +556,9 @@ def _consumers(m):
     gets one per consuming Conv / SPPF / Upsample / Detect, two per C3 (cv1 and cv2 both read it), and what its Concat gets;
     inside a C3 / SPPF the counts follow the block's structure."""
     mods = list(m.model)
-
-    def srcs(mm):
-        return [mm.i - 1 if f == -1 else (f if f >= 0 else mm.i + f) for f in ([mm.f] if isinstance(mm.f, int) else mm.f)]
-
     users = {}
     for mm in mods:
-        for s in srcs(mm):
+        for s in sources(mm):
             users.setdefault(s, []).append(mm)
 
     def E(i):
@@ -605,12 +584,10 @@ def _consumers(m):
     return cnt
 
 
-@pytest.mark.parametrize("size,B,H,W,dgrad_s2", PLANS)
-def test_plan_backward_steps(size, B, H, W, dgrad_s2, monkeypatch):
+@pytest.mark.parametrize("size,B,H,W", PLANS)
+def test_plan_backward_steps(size, B, H, W):
     """Every non-conv step of BackwardPlan.steps alone through its own closure on sentinel-filled buffers, against section
     1's references; then the accumulate flags of every gradient range in step order."""
-    if dgrad_s2:
-        monkeypatch.setenv("Y5OBB_DGRAD_S2", dgrad_s2)
     m, eng = _plan(size, B, H, W)
     plan = BackwardPlan(eng)
     g = torch.Generator(device=DEV).manual_seed(9)
@@ -618,7 +595,7 @@ def test_plan_backward_steps(size, B, H, W, dgrad_s2, monkeypatch):
     L, st = lib(), stream()
     det = m.model[-1]
     kinds = {}
-    pools = {t[1].data_ptr(): t for t in eng.layers if isinstance(t, tuple)}
+    pools = {p.cat4.data_ptr(): p for p in eng.layers if isinstance(p, _PoolLayer)}
     for tag, fn in plan.steps:
         if tag in ("dgrad", "wgrad", "zero"):
             continue
@@ -655,19 +632,8 @@ def test_plan_backward_steps(size, B, H, W, dgrad_s2, monkeypatch):
             assert torch.equal(bits(gy.view()), bits(want)), kind
             unchanged(gy.buf, before, chan_mask(gy.buf, gy.c_off, gy.C), kind)
             assert torch.equal(bits(g2.buf), bits(g2_before)), kind
-        elif tag == "zero_stuff":
-            dz, dzup = a["dz"], a["dzup"]
-            dz.copy_(torch.randn(dz.shape, device=DEV, generator=g).bfloat16())
-            dzup.fill_(OUT_SENT)
-            before = dzup.clone()
-            fn(st)
-            torch.cuda.synchronize()
-            assert torch.equal(bits(dzup[:, 0::2, 0::2]), bits(dz)), kind
-            msk = torch.zeros(dzup.shape, dtype=torch.bool, device=DEV)
-            msk[:, 0::2, 0::2] = True
-            unchanged(dzup, before, msk, kind)
         elif tag == "pool_bwd":
-            _, cat4, hh, ww, c_ = pools[a["base"]]
+            cat4, c_ = pools[a["base"]].cat4, pools[a["base"]].c
             gc = plan.gbuf[cat4.data_ptr()]
             assert gc.data_ptr() == a["gbase"]
             cat4.copy_(torch.randint(-3, 4, cat4.shape, device=DEV, generator=g).bfloat16())
@@ -725,9 +691,9 @@ def test_plan_backward_steps(size, B, H, W, dgrad_s2, monkeypatch):
                       (dg, db, torch.zeros_like(dg), torch.zeros_like(db), 0), kind)   # the plan overwrites dgamma / dbeta
         else:
             raise AssertionError(f"unexpected backward step {tag}")
-    need = {"detect_pack", "detect_bias", "upsample_bwd", "bn_bwd", "pool_bwd"} | ({"zero_stuff"} if dgrad_s2 else set())
+    need = {"detect_pack", "detect_bias", "upsample_bwd", "bn_bwd", "pool_bwd"}
     assert need <= set(kinds), kinds
-    print(f"\n{size} b{B} {H}x{W}{' ' + dgrad_s2 if dgrad_s2 else ''}: backward steps checked {kinds}")
+    print(f"\n{size} b{B} {H}x{W}: backward steps checked {kinds}")
 
     # ---- accumulate flags: every contribution to a gradient range, in step order
     ops = {}
@@ -754,9 +720,7 @@ def test_plan_backward_steps(size, B, H, W, dgrad_s2, monkeypatch):
             contrib.append((a["gbase"], 0, a["c_"], 1, "pool add"))
     cnt = _consumers(m)
     n_checked = 0
-    for lay in eng.layers:
-        if isinstance(lay, tuple):
-            continue
+    for lay in eng.conv_layers:
         gy = plan.gbuf[lay.y.buf.data_ptr()].data_ptr(), lay.y.c_off, lay.y.C
         seq = [(c[3], c[4]) for c in contrib if c[0] == gy[0] and c[1] <= gy[1] and gy[1] + gy[2] <= c[1] + c[2]]
         part = [c for c in contrib if c[0] == gy[0] and c[1] < gy[1] + gy[2] and gy[1] < c[1] + c[2]

@@ -49,15 +49,15 @@ for title, prof in (("forward", eng.prof), ("backward", eng._bwd.prof)):
     tot = sum(sum(v) for v in prof.values())
     print(title, f"{tot:.2f} ms:", "  ".join(f"{k} {sum(v):.2f} (x{len(v)})" for k, v in sorted(prof.items(), key=lambda kv: -sum(kv[1]))))
 # the ten slowest conv / wgrad / dgrad launches with their shapes
-convs = [l for l in eng.layers if not isinstance(l, tuple)]
 desc = lambda l: f"{l.x.C}->{l.z.C} k{l.mod.conv.kernel_size[0]} s{l.mod.conv.stride[0]} {l.z.H}x{l.z.W}"
-top = sorted(zip(eng.prof["conv"], convs), key=lambda t: -t[0])[:8]
+top = sorted(zip(eng.prof["conv"], eng.conv_layers), key=lambda t: -t[0])[:8]
 print("slowest fwd convs:", "; ".join(f"{t*1e3:.0f}us {desc(l)} ({l.conv.info()['flops']/t/1e9:.0f} TF/s)" for t, l in top))
 parts = eng._bwd.conv_parts
-wg = eng._bwd.prof["wgrad"][3:]   # first three are Detect levels
+nd = len(eng._bwd.det_parts)
+wg = eng._bwd.prof["wgrad"][nd:]   # the first are the Detect levels'
 top = sorted(zip(wg, parts), key=lambda t: -t[0])[:8]
 print("slowest wgrads:", "; ".join(f"{t*1e3:.0f}us {desc(p['lay'])} ({p['lay'].conv.info()['flops']/t/1e9:.0f} TF/s)" for t, p in top))
-dg = eng._bwd.prof["dgrad"][3:]
+dg = eng._bwd.prof["dgrad"][nd:]
 dl = []
 for p in parts:  # stride-2 layers launch four parity-class convs
     n = 1 if "dgrad_wp" in p else (4 if "dgrad_s2" in p else 0)

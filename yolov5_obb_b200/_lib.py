@@ -88,7 +88,6 @@ PROTOTYPES = {
     "y5obb_pack_plan_run": (c_int, [c_void_p, c_void_p]),
     "y5obb_pack_plan_destroy": (None, [c_void_p]),
     "y5obb_upsample2x_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p]),
-    "y5obb_zero_stuff2x": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
     "y5obb_maxpool5_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int,
                                    c_void_p]),
     "y5obb_add_f32_to_bf16": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),

@@ -487,22 +487,6 @@ __global__ void k_upsample2x_bwd(const __nv_bfloat16* __restrict__ gsrc, long lo
   }
 }
 
-// dst[b, 2h, 2w, :] = src[b, h, w, :], every other position zero (dst pre-zeroed once; odd positions are never written):
-// the zero-stuffed dz that turns the dgrad of a stride-2 conv into a stride-1 conv
-__global__ void k_zero_stuff2x(const __nv_bfloat16* __restrict__ src, long long src_stride, __nv_bfloat16* __restrict__ dst,
-                               long long dst_stride, long long npix, int C, int W) {
-  const int vecs = C >> 3;
-  const long long total = npix * vecs;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long p = i / vecs;
-    const int cv = (int)(i - p * vecs);
-    const long long row = p / W;
-    const int w = (int)(p - row * W);
-    *reinterpret_cast<uint4*>(dst + ((row * 2) * (2LL * W) + 2 * w) * dst_stride + cv * 8) =
-        *reinterpret_cast<const uint4*>(src + p * src_stride + cv * 8);
-  }
-}
-
 // one 5x5/s1/p2 max-pool backward step: gin[argmax window position] += gout (first maximum in row-major window order,
 // as ATen's max_pool2d_with_indices picks); fp32 accumulation buffer gin32 [npix][C]
 __global__ void k_maxpool5_bwd(const __nv_bfloat16* __restrict__ xin, long long in_stride, const float* __restrict__ gout32,
@@ -730,18 +714,6 @@ int y5obb_upsample2x_bwd(const void* gsrc, int64_t src_pix_stride, void* gdst, i
   k_upsample2x_bwd<<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const __nv_bfloat16*>(gsrc), src_pix_stride,
                                                            static_cast<__nv_bfloat16*>(gdst), dst_pix_stride, npix_dst, C,
                                                            W_dst, accumulate);
-  Y5_LAUNCH_CHECK();
-  return Y5OBB_OK;
-}
-
-int y5obb_zero_stuff2x(const void* src, int64_t src_pix_stride, void* dst, int64_t dst_pix_stride, int64_t npix_src, int C,
-                       int W_src, void* stream) {
-  if (!src || !dst || npix_src <= 0 || C <= 0 || (C & 7) || W_src <= 0 || (src_pix_stride & 7) || (dst_pix_stride & 7))
-    return Y5OBB_EINVAL;
-  const long long total = npix_src * (C / 8);
-  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  k_zero_stuff2x<<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const __nv_bfloat16*>(src), src_pix_stride,
-                                                         static_cast<__nv_bfloat16*>(dst), dst_pix_stride, npix_src, C, W_src);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
 }

@@ -16,13 +16,15 @@ BatchNorm is folded into the conv weights exactly as utils/torch_utils.py:192-21
 """
 import ctypes
 import math
+import os
 from typing import List, Optional
 
 import numpy as np
 import torch
 
 from . import _lib
-from .conv import Conv as ConvOp, Slice, WindowView, pack_weights, MODE_DETECT
+from .conv import Conv as ConvOp, Slice, pack_weights, MODE_DETECT
+from .layout import _is, route, shapes, sources, stem_weight, stem_window
 from . import yolo as Y
 
 
@@ -42,16 +44,6 @@ def _conv_params(m):
     return fold_bn(m.conv, getattr(m, "bn", None))
 
 
-def _kind(m) -> str:
-    """Module kind by class NAME, so that the reference's own modules (models/common.py, models/yolo.py,
-    torch.nn.Upsample) are accepted as well as the mirrors of yolo.py."""
-    return type(m).__name__
-
-
-def _is(m, name: str) -> bool:
-    return _kind(m) == name
-
-
 class InferenceEngine:
     def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, conv_flags: int = 0, compact_detect: bool = False,
                  det_out: Optional[torch.Tensor] = None, det_row_base: int = 0, levels=None, descale=None):
@@ -69,7 +61,6 @@ class InferenceEngine:
             raise RuntimeError(f"image size {H}x{W} must be a multiple of the max stride {smax}")
         self.device, self.B, self.H, self.W = device, B, H, W
         self.ops = []          # (callable taking stream ptr)
-        import os
         self._calls, self._graph = 0, None
         self._use_graph = os.environ.get("Y5OBB_NO_GRAPH", "0") != "1"
         self.convs: List[ConvOp] = []
@@ -79,31 +70,7 @@ class InferenceEngine:
         L = _lib.lib()
         layers = list(model.model)
         n = len(layers)
-
-        def src_of(i, f):
-            return i - 1 if f == -1 else (f if f >= 0 else i + f)
-
-        # ---- pass 1: channels and spatial size of every layer output
-        ch, hw = [0] * n, [(0, 0)] * n
-        for m in layers:
-            i = m.i
-            if _is(m, "Detect"):
-                continue
-            fs = [src_of(i, f) for f in ([m.f] if isinstance(m.f, int) else m.f)]
-            in_hw = (H, W) if i == 0 else hw[fs[0]]
-            if _is(m, "Conv"):
-                s, k, p = m.conv.stride[0], m.conv.kernel_size[0], m.conv.padding[0]
-                ch[i] = m.conv.out_channels
-                hw[i] = ((in_hw[0] + 2 * p - k) // s + 1, (in_hw[1] + 2 * p - k) // s + 1)
-            elif _is(m, "C3"):
-                ch[i], hw[i] = m.cv3.conv.out_channels, in_hw
-            elif _is(m, "SPPF"):
-                ch[i], hw[i] = m.cv2.conv.out_channels, in_hw
-            elif _is(m, "Upsample"):
-                ch[i], hw[i] = ch[fs[0]], (in_hw[0] * 2, in_hw[1] * 2)
-            elif _is(m, "Concat"):
-                ch[i], hw[i] = sum(ch[f] for f in fs), in_hw
-                assert all(hw[f] == in_hw for f in fs)
+        ch, hw = shapes(layers, H, W)
 
         # ---- liveness: backwards from the inputs of the kept Detect levels (a pruned level's head is not emitted)
         self.levels = tuple(range(det.nl)) if levels is None else tuple(sorted(set(int(l) for l in levels)))
@@ -114,7 +81,7 @@ class InferenceEngine:
         for m in reversed(layers[:-1]):
             if m.i in need:
                 live[m.i] = True
-                need.update(src_of(m.i, f) for f in ([m.f] if isinstance(m.f, int) else m.f))
+                need.update(sources(m))
 
         arena = {"buf": None, "used": 0}
 
@@ -132,49 +99,10 @@ class InferenceEngine:
             arena["used"] += n_al
             return t
 
-        # ---- pass 2: who feeds a concat
-        feeds = {}
-        cat_buf = {}
-        for m in layers:
-            if _is(m, "Concat"):
-                cat_buf[m.i] = new(hw[m.i][0], hw[m.i][1], ch[m.i])
-                off = 0
-                for f in m.f:
-                    s = src_of(m.i, f)
-                    if s in feeds:
-                        raise RuntimeError("a layer feeding two Concats is not in the shipped yamls")
-                    feeds[s] = (m.i, off)
-                    off += ch[s]
-        out: List[Optional[Slice]] = [None] * n
-        up_of = {}  # producer conv index -> Slice receiving the up-sampled copy
-        for m in layers:
-            i = m.i
-            if _is(m, "Detect"):
-                continue
-            if _is(m, "Concat"):
-                out[i] = Slice.full(cat_buf[i])
-            elif _is(m, "Upsample"):
-                if i not in feeds:
-                    raise RuntimeError("nn.Upsample must feed a Concat (v6.0 head pattern)")
-                j, off = feeds[i]
-                src = src_of(i, m.f)
-                if not _is(layers[src], "Conv"):
-                    raise RuntimeError("nn.Upsample must follow a Conv (v6.0 head pattern)")
-                up_of[src] = Slice(cat_buf[j], off, ch[i])
-                out[i] = up_of[src]
-            elif i in feeds:
-                j, off = feeds[i]
-                out[i] = Slice(cat_buf[j], off, ch[i])
-            else:
-                out[i] = Slice.full(new(hw[i][0], hw[i][1], ch[i]))
-
+        out, up_of = route(layers, ch, hw, new)
         self.out_slices = out   # per top-level layer: where its output lives (tests read them for teacher-forced parity)
-        import os
-        dbg_no_res = os.environ.get("Y5OBB_DEBUG_NO_RES") == "1"  # timing experiments only (wrong results)
 
         def add_conv(x, w, b, k, s, p, act, dst: Optional[Slice] = None, res=None, out2x=None, detd=None):
-            if dbg_no_res:
-                res = None
             wp, bp = pack_weights(w.cpu(), b.cpu(), MODE_DETECT if detd else 0, detd["no"] if detd else 0)   # packed on the host
             if act and not detd:
                 bp = bp * 0.5   # the SiLU epilogue wants 0.5 * bias (Y5OBB_CONV_BIAS_HALVED)
@@ -202,7 +130,7 @@ class InferenceEngine:
             if not live[i]:
                 continue
             cur[0] = i
-            fs = [src_of(i, f) for f in ([m.f] if isinstance(m.f, int) else m.f)]
+            fs = sources(m)
             if _is(m, "Conv"):
                 w, b = _conv_params(m)
                 k, s, p = m.conv.kernel_size[0], m.conv.stride[0], m.conv.padding[0]
@@ -210,17 +138,7 @@ class InferenceEngine:
                 if i == 0:
                     if (k, s, p, w.shape[1]) != (6, 2, 2, 3):
                         raise RuntimeError("layer 0 must be the v6.0 stem Conv(3, c, 6, 2, 2)")
-                    # w2[co, (dy*2+dx)*3 + c, ty, tx] = w[co, c, 2*ty+dy, 2*tx+dx]   (3x3/s1/p1 over the s2d image)
-                    w2 = torch.zeros((w.shape[0], 16, 3, 3))
-                    for dy in range(2):
-                        for dx in range(2):
-                            w2[:, (dy * 2 + dx) * 3:(dy * 2 + dx) * 3 + 3] = w[:, :, dy::2, dx::2]
-                    # w3[co, tx*16 + ch, ty, 0] = w2[co, ch, ty, tx]   (3x1 over 48-channel windows)
-                    w3 = w2.permute(0, 3, 1, 2).reshape(w.shape[0], 48, 3, 1).contiguous()
-                    Wp = W // 2 + 2
-                    win = WindowView(buf=self.x_s2d, ptr=self.x_s2d.data_ptr(), pix_stride=16, row_stride=Wp * 16,
-                                     img_stride=(H // 2) * Wp * 16, B=B, H=H // 2, W=W // 2, C=48, hbm_c=16)
-                    add_conv(win, w3, b, (3, 1), 1, (1, 0), act, out[i])
+                    add_conv(stem_window(self.x_s2d), stem_weight(w), b, (3, 1), 1, (1, 0), act, out[i])
                 else:
                     add_conv(out[fs[0]], w, b, k, s, p, act, out[i], out2x=up_of.get(i))
             elif _is(m, "C3"):

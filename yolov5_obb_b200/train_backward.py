@@ -5,7 +5,7 @@ as a fixed sequence of sm_90a kernel launches.
 Per Conv module (y = [res +] silu(bn(conv(x))), reverse order):
    gy (+ 2x-up-sampled copy's gradient folded in)  --y5obb_bn_silu_bwd-->  dz, dgamma, dbeta, residual pass-through
    dz, x  --y5obb_wgrad (both read in place, NHWC)-->  dW (tensor cores, split-K)
-   dz     --conv_tc_kernel with transposed / flipped weights (dgrad; stride 2: over the zero-stuffed dz)-->  gx (+=)
+   dz     --conv_tc_kernel with transposed / flipped weights (dgrad; stride 2: one conv per output-pixel parity)-->  gx (+=)
 Gradient buffers mirror the activation buffers; whether a contribution overwrites or accumulates is decided
 statically when the plan is built (first writer of a channel range overwrites).
 Parameter gradients land in views of ONE flat fp32 buffer owned by the plan (run() returns it); the autograd
@@ -18,7 +18,8 @@ import torch
 
 from . import _lib
 from .conv import Conv as ConvOp, Slice, pack_weights, tiling, MODE_DETECT
-from .train_engine import flat_layout
+from .layout import stem_grad
+from .train_engine import _PoolLayer, flat_layout
 from .train_ops import Wgrad
 
 
@@ -83,8 +84,7 @@ class BackwardPlan:
         written = _Written()
         det = eng.model.model[-1]
 
-        # activation-sized buffers come from the engine's allocator (its arena when one is reserved, train_engine.TrainArena);
-        # `zero=True` marks the ones a launch relies on being zero where nothing writes them
+        # activation-sized buffers come from the engine's allocator (its arena when one is reserved, train_engine.TrainArena)
         carve = eng._carver.take
 
         def gslice(s: Slice) -> Slice:
@@ -98,8 +98,8 @@ class BackwardPlan:
             self.keep.append(t)
             return t
 
-        def bf(*shape, zero=False):
-            t = carve(shape, torch.bfloat16, zero=zero)
+        def bf(*shape):
+            t = carve(shape, torch.bfloat16)
             self.keep.append(t)
             return t
 
@@ -173,8 +173,8 @@ class BackwardPlan:
         # ---------------- conv layers, reverse ----------------
         self.conv_parts = []
         for lay in reversed(eng.layers):
-            if isinstance(lay, tuple):
-                _, cat4, hh, ww, c_ = lay
+            if isinstance(lay, _PoolLayer):
+                cat4, hh, ww, c_ = lay.cat4, lay.h, lay.w, lay.c
                 gc = gslice(Slice.full(cat4))
                 npix = B * hh * ww
                 t2, t1, t0 = f32(npix * c_), f32(npix * c_), f32(npix * c_)
@@ -231,30 +231,20 @@ class BackwardPlan:
 
             # ---- wgrad (straight from the NHWC buffers)
             x = lay.x
-            if lay.stem:  # the forward's view: a 3x1 conv over 48-channel windows (3 horizontal taps x 16 s2d channels)
-                Wp = eng.W // 2 + 2
-                Hi, Wi, Cin_w = eng.H // 2, eng.W // 2, 48
-                kw_, sw_, pw_ = (3, 1), 1, (1, 0)
-                x_ptr, x_ps, x_keep = eng.x_s2d.data_ptr(), 16, eng.x_s2d
-                x_strides = (Wp * 16, (eng.H // 2) * Wp * 16)
-            else:
-                Hi, Wi, Cin_w = x.H, x.W, x.C
-                kw_, sw_, pw_ = k, s, p
-                x_ptr, x_ps, x_keep = x.ptr, x.pix_stride, x.buf
-                x_strides = (0, 0)
-            ntap = kw_[0] * kw_[1] if isinstance(kw_, tuple) else kw_ * kw_
-            if lay.stem:  # gradient over the space-to-depth form, re-mapped to [Cout,3,6,6] at the end of run()
-                dw = f32(3 * Cout * 48)
+            if lay.stem:  # the forward's window view: a 3x1 conv over 48-channel windows (3 horizontal taps x 16 s2d channels)
+                dw = f32(3 * Cout * x.C)   # gradient over the space-to-depth form, re-mapped to [Cout,3,6,6] at the end of run()
                 part["stem_dw"] = dw
                 add("zero", lambda st, dw=dw: dw.zero_())
-                wg = Wgrad(dz.data_ptr(), Cout, x_ptr, x_ps, dw, B, Cout, Hh, Ww, Cin_w, Hi, Wi, kw_, sw_, pw_, keep=(dz, x_keep),
-                           x_strides=x_strides)
+                wg = Wgrad(dz.data_ptr(), Cout, x.ptr, x.pix_stride, dw, B, Cout, Hh, Ww, x.C, x.H, x.W, (3, 1), 1, (1, 0),
+                           keep=(dz, x.buf), x_strides=(x.row_stride, x.img_stride))
+                ntap = 3
             else:
-                wg = Wgrad(dz.data_ptr(), Cout, x_ptr, x_ps, grad_of(conv.weight), B, Cout, Hh, Ww, Cin_w, Hi, Wi, kw_, sw_, pw_,
-                           keep=(dz, x_keep, self.flat), param_layout=True)
+                wg = Wgrad(dz.data_ptr(), Cout, x.ptr, x.pix_stride, grad_of(conv.weight), B, Cout, Hh, Ww, x.C, x.H, x.W, k, s, p,
+                           keep=(dz, x.buf, self.flat), param_layout=True)
+                ntap = k * k
             self.keep.append(wg)
             part["wgrad"] = wg
-            self.flops += 2.0 * npix * Cout * Cin_w * ntap
+            self.flops += 2.0 * npix * Cout * x.C * ntap
             add("wgrad", lambda st, wg=wg: wg.run(st))
 
             # ---- dgrad
@@ -268,10 +258,13 @@ class BackwardPlan:
                     part["dgrad_wp"] = wp
                     part["dgrad_ops"].append(op)
                     self.keep.append(op)
-                elif k == 3 and p == 1 and x.H % 2 == 0 and x.W % 2 == 0 and os.environ.get("Y5OBB_DGRAD_S2", "phase") == "phase":
+                else:
+                    if (k, s, p) != (3, 2, 1) or x.H % 2 or x.W % 2:
+                        raise RuntimeError(f"the data gradient of a k{k} s{s} p{p} conv on a {x.H}x{x.W} input is not planned "
+                                           "(stride 2 is planned for 3x3 / pad 1 on an even input)")
                     # Output pixels of parity (ph, pw) only see the taps of matching parity: four 1- / 2-tap stride-1
                     # convolutions of dz, each written to every other pixel of gx - 9 tap-GEMMs per 4 outputs instead of
-                    # the 36 of the zero-stuffed form.
+                    # the 36 of a stride-1 conv over the zero-stuffed dz.
                     acc = written.contribute(gx)
                     ps = gx.pix_stride
                     part["dgrad_s2"] = []
@@ -287,14 +280,6 @@ class BackwardPlan:
                             part["dgrad_s2"].append((ph * 2 + pw, wp))
                             part["dgrad_ops"].append(op)
                             self.keep.append(op)
-                else:
-                    dzup = bf(B, x.H, x.W, Cout, zero=True)   # odd positions: zero, never written by zero_stuff2x
-                    add("zero_stuff", lambda st, dz=dz, dzup=dzup, npix=npix, C=Cout, W=Ww:
-                                      _lib.check(L.y5obb_zero_stuff2x(dz.data_ptr(), C, dzup.data_ptr(), C, npix, C, W, st), "zero_stuff"))
-                    op, wp = add_dgrad(Slice.full(dzup), w_d, k, k - 1 - p, gx, "dgrad s2")
-                    part["dgrad_wp"] = wp
-                    part["dgrad_ops"].append(op)
-                    self.keep.append(op)
         self.refresh()
 
     # ------------------------------------------------------------------------------------------
@@ -383,11 +368,6 @@ class BackwardPlan:
                 mi, bn = part["mi"], part["bn"]
                 self.pgrad[mi.bias].copy_(part["s1"].view(det.na, bn)[:, :det.no].reshape(-1))
             for part in self.conv_parts:
-                if "stem_dw" in part:  # dw[ty][co][tx * 16 + (dy*2+dx)*3 + c] is the gradient of w[co, c, 2ty+dy, 2tx+dx]
-                    conv = part["lay"].mod.conv
-                    dw = part["stem_dw"].view(3, conv.out_channels, 3, 16).permute(1, 3, 0, 2)  # [co, ch16, ty, tx]
-                    g = self.pgrad[conv.weight]
-                    for dy in range(2):
-                        for dx in range(2):
-                            g[:, :, dy::2, dx::2].copy_(dw[:, (dy * 2 + dx) * 3:(dy * 2 + dx) * 3 + 3])
+                if "stem_dw" in part:
+                    stem_grad(part["stem_dw"], self.pgrad[part["lay"].mod.conv.weight])
         return self.flat

@@ -7,13 +7,13 @@ Differences from the inference plan (engine.py): BN is not folded, nothing is up
 every activation), cv1/cv2 of a C3 run as separate GEMMs (each has its own BatchNorm), and the raw conv output z
 of every layer is stored next to its activated output y."""
 import weakref
-from typing import Dict, List, Optional
+from typing import List, NamedTuple, Optional, Union
 
 import torch
 
 from . import _lib
-from .conv import Conv as ConvOp, Slice, WindowView, pack_weights, MODE_DETECT
-from .engine import _is
+from .conv import Conv as ConvOp, Slice, pack_weights, MODE_DETECT
+from .layout import _is, route, shapes, sources, stem_weight, stem_window
 
 
 def flat_layout(params):
@@ -64,7 +64,7 @@ class _Carver:
         self.arena, self.device, self.off = arena, device, 0
         self.zero = []   # regions the plan relies on being zero
 
-    def take(self, shape, dtype, zero: bool = False) -> torch.Tensor:
+    def take(self, shape, dtype) -> torch.Tensor:
         n = 1
         for s in shape:
             n *= int(s)
@@ -77,10 +77,7 @@ class _Carver:
         if self.off > self.arena.nbytes:
             raise RuntimeError(f"training plan needs more than the {self.arena.nbytes} bytes of the reserved arena: "
                                "reserve it for the largest batch and image size (Model.reserve_train_arena)")
-        t = self.arena.buf[off:off + nbytes].view(dtype).view(tuple(shape))
-        if zero:
-            self.zeroed(t)
-        return t
+        return self.arena.buf[off:off + nbytes].view(dtype).view(tuple(shape))
 
     def zeroed(self, t: torch.Tensor):
         """Register a view of an arena buffer that must read as zero whenever the plan runs (and zero it now)."""
@@ -106,6 +103,16 @@ class _BNLayer:
         self.act = isinstance(mod.act, torch.nn.SiLU)
 
 
+class _PoolLayer(NamedTuple):
+    """SPPF's three chained 5x5 max-pools (models/common.py:190-196): channels [0, c) of cat4 [B, h, w, 4c] into
+    [c, 2c), [2c, 3c) and [3c, 4c).  Still the tuple ("pool", cat4, h, w, c) for code that unpacks the entry."""
+    kind: str
+    cat4: torch.Tensor
+    h: int
+    w: int
+    c: int
+
+
 class TrainEngine:
     def __init__(self, model, B: int, H: int, W: int, device, in_hw=None, arena: Optional[TrainArena] = None,
                  carver: Optional[_Carver] = None):
@@ -126,89 +133,29 @@ class TrainEngine:
         self._carver = carver if carver is not None else _Carver(arena, device)
         mem0 = torch.cuda.memory_allocated(device)
         self.model = model
-        self.layers: List[_BNLayer] = []
+        self.layers: List[Union[_BNLayer, _PoolLayer]] = []   # in launch order
         self.pre_ops, self.keep = [], []
         self.flops = 0.0
         L = _lib.lib()
         self._L = L
         mods = list(model.model)
-        n = len(mods)
-
-        def src_of(i, f):
-            return i - 1 if f == -1 else (f if f >= 0 else i + f)
-
-        ch, hw = [0] * n, [(0, 0)] * n
-        for m in mods:
-            i = m.i
-            if _is(m, "Detect"):
-                continue
-            fs = [src_of(i, f) for f in ([m.f] if isinstance(m.f, int) else m.f)]
-            in_hw = (H, W) if i == 0 else hw[fs[0]]
-            if _is(m, "Conv"):
-                s, k, p = m.conv.stride[0], m.conv.kernel_size[0], m.conv.padding[0]
-                ch[i], hw[i] = m.conv.out_channels, ((in_hw[0] + 2 * p - k) // s + 1, (in_hw[1] + 2 * p - k) // s + 1)
-            elif _is(m, "C3"):
-                ch[i], hw[i] = m.cv3.conv.out_channels, in_hw
-            elif _is(m, "SPPF"):
-                ch[i], hw[i] = m.cv2.conv.out_channels, in_hw
-            elif _is(m, "Upsample"):
-                ch[i], hw[i] = ch[fs[0]], (in_hw[0] * 2, in_hw[1] * 2)
-            elif _is(m, "Concat"):
-                ch[i], hw[i] = sum(ch[f] for f in fs), in_hw
+        ch, hw = shapes(mods, H, W)
 
         def new(h, w, c):
             t = self._carver.take((B, h, w, c), torch.bfloat16)
             self.keep.append(t)
             return t
 
-        feeds, cat_buf = {}, {}
-        for m in mods:
-            if _is(m, "Concat"):
-                cat_buf[m.i] = new(hw[m.i][0], hw[m.i][1], ch[m.i])
-                off = 0
-                for f in m.f:
-                    s = src_of(m.i, f)
-                    feeds[s] = (m.i, off)
-                    off += ch[s]
-        out: List[Optional[Slice]] = [None] * n
-        up_of: Dict[int, Slice] = {}
-        for m in mods:
-            i = m.i
-            if _is(m, "Detect"):
-                continue
-            if _is(m, "Concat"):
-                out[i] = Slice.full(cat_buf[i])
-            elif _is(m, "Upsample"):
-                j, off = feeds[i]
-                src = src_of(i, m.f)
-                if not _is(mods[src], "Conv"):
-                    raise RuntimeError("nn.Upsample must follow a Conv (v6.0 head pattern)")
-                up_of[src] = Slice(cat_buf[j], off, ch[i])
-                out[i] = up_of[src]
-            elif i in feeds:
-                j, off = feeds[i]
-                out[i] = Slice(cat_buf[j], off, ch[i])
-            else:
-                out[i] = Slice.full(new(hw[i][0], hw[i][1], ch[i]))
+        out, up_of = route(mods, ch, hw, new)
 
         def add(mod, x, dst: Slice, res=None, y2x=None, stem=False):
             conv = mod.conv
-            k, s, p = conv.kernel_size[0], conv.stride[0], conv.padding[0]
-            hh, ww = dst.H, dst.W
-            z = Slice.full(new(hh, ww, conv.out_channels))
+            k, s, p = ((3, 1), 1, (1, 0)) if stem else (conv.kernel_size[0], conv.stride[0], conv.padding[0])
+            z = Slice.full(new(dst.H, dst.W, conv.out_channels))
             lay = _BNLayer(mod, x, z, dst, res, y2x)
             w = conv.weight.detach().float()
-            if stem:
-                w2 = torch.zeros((w.shape[0], 16, 3, 3), device=w.device)
-                for dy in range(2):
-                    for dx in range(2):
-                        w2[:, (dy * 2 + dx) * 3:(dy * 2 + dx) * 3 + 3] = w[:, :, dy::2, dx::2]
-                w = w2.permute(0, 3, 1, 2).reshape(w.shape[0], 48, 3, 1).contiguous()
-                wp, bp = pack_weights(w, None)
-                lay.conv = ConvOp(x, wp, bp, w.shape[0], (3, 1), 1, (1, 0), False, out=z)
-            else:
-                wp, bp = pack_weights(w, None)
-                lay.conv = ConvOp(x, wp, bp, w.shape[0], k, s, p, False, out=z)
+            wp, bp = pack_weights(stem_weight(w) if stem else w, None)
+            lay.conv = ConvOp(x, wp, bp, w.shape[0], k, s, p, False, out=z)
             lay.wp, lay.stem = wp, stem
             self.flops += lay.conv.info()["flops"]
             self.layers.append(lay)
@@ -222,13 +169,10 @@ class TrainEngine:
             i = m.i
             if _is(m, "Detect"):
                 break
-            fs = [src_of(i, f) for f in ([m.f] if isinstance(m.f, int) else m.f)]
+            fs = sources(m)
             if _is(m, "Conv"):
                 if i == 0:
-                    Wp = W // 2 + 2
-                    win = WindowView(buf=self.x_s2d, ptr=self.x_s2d.data_ptr(), pix_stride=16, row_stride=Wp * 16,
-                                     img_stride=(H // 2) * Wp * 16, B=B, H=H // 2, W=W // 2, C=48, hbm_c=16)
-                    add(m, win, out[i], stem=True)
+                    add(m, stem_window(self.x_s2d), out[i], stem=True)
                 else:
                     add(m, out[fs[0]], out[i], y2x=up_of.get(i))
             elif _is(m, "C3"):
@@ -253,7 +197,7 @@ class TrainEngine:
                 hh, ww = hw[i]
                 cat4 = new(hh, ww, 4 * c_)
                 add(m.cv1, x, Slice(cat4, 0, c_))
-                self.layers.append(("pool", cat4, hh, ww, c_))
+                self.layers.append(_PoolLayer("pool", cat4, hh, ww, c_))
                 add(m.cv2, Slice.full(cat4), out[i])
 
         # Detect: raw logits per level, fp32 [B, na, H, W, no]
@@ -274,13 +218,14 @@ class TrainEngine:
             self.det_out.append(o)
             self.det_convs.append(cv)
         self.out_slices = out
+        self.conv_layers = [lay for lay in self.layers if isinstance(lay, _BNLayer)]
         self._bwd, self._pack, self._pack_has_bwd = None, None, False
         self.prof = None  # set to {} to collect per-kernel-kind device times (ms) during forward()
         import os
         self.use_graph = os.environ.get("Y5OBB_NO_GRAPH", "0") != "1"
         self._graphs = {}
-        self._nbt = [lay.mod.bn.num_batches_tracked for lay in self.layers if not isinstance(lay, tuple)]
-        cmax = max([lay.z.C for lay in self.layers if not isinstance(lay, tuple)] + [det.na * 256])
+        self._nbt = [lay.mod.bn.num_batches_tracked for lay in self.conv_layers]
+        cmax = max([lay.z.C for lay in self.conv_layers] + [det.na * 256])
         self.scratch = torch.zeros(int(L.y5obb_bn_scratch_floats(cmax)), dtype=torch.float32, device=device)  # reductions
         # device bytes this plan holds outside the arena (BatchNorm vectors, packed weights, scratch; later the backward
         # plan's and the captured graphs'): with an arena, what each additional training shape costs
@@ -298,13 +243,7 @@ class TrainEngine:
                 t.zero_()
             a.owner = weakref.ref(self)
 
-    @staticmethod
-    def _stem_weight(w):
-        w2 = torch.zeros((w.shape[0], 16, 3, 3), device=w.device)
-        for dy in range(2):
-            for dx in range(2):
-                w2[:, (dy * 2 + dx) * 3:(dy * 2 + dx) * 3 + 3] = w[:, :, dy::2, dx::2]
-        return w2.permute(0, 3, 1, 2).reshape(w.shape[0], 48, 3, 1).contiguous()
+    _stem_weight = staticmethod(stem_weight)   # layout.stem_weight under the name TrainEngine's callers use
 
     def refresh_weights(self):
         """Re-pack the (updated) fp32 parameters into the bf16 buffers the TMA descriptors point at — after every
@@ -313,9 +252,7 @@ class TrainEngine:
             from .train_ops import PackPlan, PACK_FWD, PACK_STEM, PACK_DETECT, PACK_DETECT_BIAS
             det = self.model.model[-1]
             ent = []
-            for lay in self.layers:
-                if isinstance(lay, tuple):
-                    continue
+            for lay in self.conv_layers:
                 ent.append((PACK_STEM if lay.stem else PACK_FWD, lay.mod.conv.weight.data, lay.wp, 0, 0))
             for l, cv in enumerate(self.det_convs):
                 bn = cv._keep[1].shape[1] // det.na
@@ -391,9 +328,9 @@ class TrainEngine:
             else:
                 run("s2d", lambda: L.y5obb_stem_s2d(x.data_ptr(), self.x_s2d.data_ptr(), self.B, self.H, self.W, 1, st))
             for lay in self.layers:
-                if isinstance(lay, tuple):
-                    _, cat4, hh, ww, c_ = lay
-                    run("pool", lambda: L.y5obb_sppf_pool(cat4.data_ptr(), cat4.shape[3], self.B, hh, ww, c_, st))
+                if isinstance(lay, _PoolLayer):
+                    run("pool", lambda: L.y5obb_sppf_pool(lay.cat4.data_ptr(), lay.cat4.shape[3], self.B, lay.h, lay.w, lay.c,
+                                                          st))
                     continue
                 run("conv", lambda: L.y5obb_conv_run(lay.conv._h, st))
                 z, y = lay.z, lay.y

@@ -15,6 +15,8 @@ from pathlib import Path
 import torch
 import torch.nn as nn
 
+from .layout import shapes
+
 # ---------------------------------------------------------------------------------------------
 # configuration (values of models/yolov5{n,s,m,l,x}.yaml and models/hub/yolov5{n,s,m,l,x}6.yaml, generated rather than stored)
 # ---------------------------------------------------------------------------------------------
@@ -266,20 +268,8 @@ class Model(nn.Module):
         self._generation = getattr(self, "_generation", 0) + 1
 
     def _strides(self):
-        s, out = [], {}
-        for m in self.model:
-            f = m.f if isinstance(m.f, int) else m.f[0]
-            src = (m.i - 1 if f == -1 else f)
-            cur = out.get(src, 1.0) if m.i > 0 else 1.0
-            if isinstance(m, Conv) and m.conv.stride[0] == 2:
-                cur *= 2
-            elif isinstance(m, Upsample):
-                cur /= 2
-            out[m.i] = cur
-        det = self.model[-1]
-        for j in det.f:
-            s.append(float(out[j]))
-        return s
+        _, hw = shapes(list(self.model), 256, 256)
+        return [256 / hw[j][0] for j in self.model[-1].f]
 
     def _initialize_biases(self, cf=None):  # models/yolo.py:223-232 (touches the 180 theta channels too)
         m = self.model[-1]
