@@ -122,6 +122,8 @@ typedef struct y5obb_conv y5obb_conv_t;
                                       first global-memory access; also switched off by the environment variable Y5OBB_NO_PDL=1) */
 #define Y5OBB_CONV_ONE_CTA 64      /* flags: one CTA per SM even for N tiles <= 96 (default: two when the plan fits half of
                                       the shared memory; debug / A-B comparison) */
+#define Y5OBB_CONV_DETECT_GENERIC 128  /* flags: compact Detect records (det_decode 2) through the shared epilogue instead of
+                                      the records epilogue (default; bit-identical records); A-B comparison */
 
 typedef struct {
   const void* in;            /* bf16 NHWC slice */

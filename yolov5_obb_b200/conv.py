@@ -122,6 +122,7 @@ class WindowView:
 
 NO_ROWSHIFT, NO_RESIDENT, NO_PAIRW, BIAS_HALVED = 1, 2, 4, 8
 ONE_CTA = 64   # one CTA per SM for every instantiation (A/B comparison of the two-CTA plans)
+DETECT_GENERIC = 128   # compact Detect records through the shared epilogue (A/B comparison of the records epilogue)
 
 
 class Conv:

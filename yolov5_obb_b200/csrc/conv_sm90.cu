@@ -158,13 +158,27 @@ __device__ __forceinline__ uint64_t desc_from(uint32_t lo, uint32_t hi) {
   return d;
 }
 
+// Y5OBB_DETECT_PROBE (tools/time_detect.py builds it into a library of its own): thread 0 of every CTA of a compact-record
+// Detect launch stamps clock64 at each phase of its first PROBE_TILES tiles; y5obb_detect_probe copies the stamps out.
+enum ProbePhase : int { PH_TILE = 0, PH_FULL, PH_MMA, PH_ARGMAX, PH_STAGED, PH_STORED, PROBE_PHASES };
+#ifdef Y5OBB_DETECT_PROBE
+constexpr int PROBE_CTAS = 264, PROBE_TILES = 64;
+__device__ long long g_probe[PROBE_CTAS][PROBE_TILES][PROBE_PHASES];
+__device__ __forceinline__ void probe(const ConvK& p, int ti, int ph) {
+  if (p.mode == MODE_DETECT && p.det_decode == 2 && threadIdx.x == 0 && blockIdx.x < PROBE_CTAS && ti < PROBE_TILES)
+    g_probe[blockIdx.x][ti][ph] = clock64();
+}
+#else
+__device__ __forceinline__ void probe(const ConvK&, int, int) {}
+#endif
+
 // ---- epilogue of one tile for one consumer warp ----------------------------------------------------------------------
 // The warp owns 16 pixel rows (row0 .. row0 + 15 of the tile).  wgmma's accumulator layout gives thread `lane` the rows
 // row0 + lane / 4 (+ 8) and the column pairs 8 j + 2 (lane % 4) (+ 1).  Each 64-column block is activated in registers,
 // staged through shared memory as [16 rows][64] fp32 and leaves in 16-byte vectors per pixel.
 template <int NI>
 __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg, const float* bias_s,
-                                         int row0, int lane) {
+                                         int row0, int lane, int ti) {
   const int q = lane & 3, r = lane >> 2;
   constexpr int PITCH = stg_pitch(NI), VECS = stg_cols(NI) / 8;  // 8-column vectors per staged row
   float* theta_s = stg + 16 * PITCH;
@@ -206,6 +220,7 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
       }
       if (q == 0) theta_s[r + 8 * i] = (float)bk[i];
     }
+    probe(p, ti, PH_ARGMAX);
   }
   const int ncols = (det && p.det_decode == 2) ? p.det_rec_w : nvalid;  // columns that leave the kernel
 #pragma unroll
@@ -234,6 +249,7 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
       }
     }
     __syncwarp();
+    probe(p, ti, PH_STAGED);
     // (2) 16 rows x (up to) 64 columns leave in vectors
     if (!det) {
       for (int v = lane; v < 16 * VECS; v += 32) {
@@ -314,9 +330,128 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
     }
     __syncwarp();
   }
+  probe(p, ti, PH_STORED);
 }
 
+// ---- compact-record Detect epilogue (det_decode 2, det_rec_w <= 64) -----------------------------------------------------
+// The same record, bit for bit, as epilogue<NI>'s records branch: the same fp32 expressions on the same accumulators, only
+// scheduled differently.  Thread `lane` holds rows row0 + r (+ 8) and columns 8 j + 2 q (+ 1), q = lane % 4, r = lane / 4.
+//
+// bt_s, NI floats behind the bias in shared memory, holds the CTA's current anchor's theta biases: bias[col] for the 180
+// theta bins (nfix <= col < det_no), -inf for every other column.  acc + (-inf) is -inf, or NaN for an infinite acc, and
+// neither is ever > best, so the arg-max needs no column test: it is straight-line load / add / compare / select code.
+// (Registers would be faster still, but the accumulators already take 112 of the 168 that ptxas may allocate.)
+//
+// The record (cx, cy, w, h, obj, cls[nc], theta index, zero padding) of each row is built in registers and written once to
+// the warp's staging buffer as [16 rows][det_rec_w] fp32 - the layout of 16 consecutive output rows.  Rows that are
+// consecutive pixels of one image row (all 16 when the tile spans whole image rows, Wt == Wout) are consecutive records of
+// [B, A, rec_w], so each run of them leaves in one cp.async.bulk store.  The store reads the staging buffer asynchronously;
+// the next tile's epilogue waits for that read before it writes the buffer again, so the store overlaps the next tile's MMAs.
 template <int NI>
+__device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], const float* bt_s,
+                                                 float* stg, const float* bias_s, int row0, int lane, int ti) {
+  const int q = lane & 3, r = lane >> 2;
+  const int nfix = p.det_no - 180, rw = p.det_rec_w;
+  // (1) theta: the first maximum of acc + bias over the 180 bins.  Per thread in increasing column order (strict >), then
+  // across the quad (larger value, or equal value and smaller column) - epilogue<NI>'s order and tie rule.  bk holds the
+  // column; nfix (bin 0) is what a row without any finite logit reports, as there.
+  float best[2] = {-INFINITY, -INFINITY};
+  int bk[2] = {nfix, nfix};
+  const uint32_t bt_u = ptx::smem_u32(bt_s + 2 * q);
+#pragma unroll
+  for (int j = 0; j < NI / 8; ++j) {
+    const float2 bt = ptx::ld_shared_v2(bt_u + 32u * j);
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float v = acc[4 * j + 2 * i + k] + (k ? bt.y : bt.x);
+        const bool take = v > best[i];
+        best[i] = take ? v : best[i];
+        bk[i] = take ? 8 * j + 2 * q + k : bk[i];
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best[i], off);
+      const int ok = __shfl_xor_sync(0xffffffffu, bk[i], off);
+      const bool take = ob > best[i] || (ob == best[i] && ok < bk[i]);
+      best[i] = take ? ob : best[i];
+      bk[i] = take ? ok : bk[i];
+    }
+  probe(p, ti, PH_ARGMAX);
+
+  // (2) sigmoid and decode in registers, straight into the staged records
+  const int a = c.nt;
+  float px[2], py[2];  // the grid cell (w, h) of the thread's two rows
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int tr = row0 + r + 8 * i;
+    const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+    px[i] = (float)(c.w0 + (tr - hl * p.Wt));
+    py[i] = (float)(c.h0 + hl);
+  }
+  const float* bias = bias_s + c.n0;
+  const uint32_t stg_u = ptx::smem_u32(stg);
+  ptx::tma_store_wait_read<0>();  // the previous tile's bulk stores have read the staging buffer
+  __syncwarp();
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {  // det_rec_w <= 64
+    const int col = 8 * j + 2 * q;
+    if (8 * j >= rw) break;
+    if (col >= rw) continue;
+    const float2 b = col < nfix ? ptx::ld_shared_v2(ptx::smem_u32(bias + col)) : make_float2(0.0f, 0.0f);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float f0 = sigmoid_fast(acc[4 * j + 2 * i] + b.x), f1 = sigmoid_fast(acc[4 * j + 2 * i + 1] + b.y);
+      if (j == 0 && q < 2) {  // xy, wh (models/yolo.py)
+        if (q == 0) {
+          f0 = (f0 * 2.0f - 0.5f + px[i]) * p.det_stride;
+          f1 = (f1 * 2.0f - 0.5f + py[i]) * p.det_stride;
+        } else {
+          f0 = (f0 * 2.0f) * (f0 * 2.0f) * p.det_anchor[2 * a];
+          f1 = (f1 * 2.0f) * (f1 * 2.0f) * p.det_anchor[2 * a + 1];
+        }
+        if (p.det_descale) {  // _descale_pred, as in epilogue<NI>
+          f0 = __fmul_rn(f0, p.det_inv_scale);
+          f1 = __fmul_rn(f1, p.det_inv_scale);
+          if (q == 0 && p.det_flip_w > 0.0f) f0 = __fsub_rn(p.det_flip_w, f0);
+        }
+      }
+      const float th = (float)(bk[i] - nfix);
+      if (col >= nfix) f0 = col == nfix ? th : 0.0f;
+      if (col + 1 >= nfix) f1 = col + 1 == nfix ? th : 0.0f;
+      ptx::st_shared_v2(stg_u + (uint32_t)(((r + 8 * i) * rw + col) * 4), f0, f1);
+    }
+  }
+  ptx::fence_proxy_async();  // the staged records, written through the generic proxy, are read by the bulk copy
+  __syncwarp();
+  probe(p, ti, PH_STAGED);
+
+  // (3) lane l < 16 describes row l: its output row, and whether a run of consecutive output rows starts there
+  const int l = lane & 15;
+  const int tr = row0 + l;
+  const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+  const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
+  const bool valid = lane < 16 && h < p.Hout && w < p.Wout;
+  const long long orow = (long long)c.b * p.det_rows_per_image + p.det_row_off + ((long long)a * p.Hout + h) * p.Wout + w;
+  const long long prev = __shfl_up_sync(0xffffffffu, orow, 1);
+  const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+  const bool start = valid && (l == 0 || !((vmask >> (l - 1)) & 1u) || prev + 1 != orow);
+  const uint32_t smask = __ballot_sync(0xffffffffu, start);
+  if (start) {
+    const uint32_t brk = ((smask | ~vmask) & (0xFFFFFFFEu << l)) | (1u << 16);  // the first row after l that ends the run
+    const int len = __ffs(brk) - 1 - l;
+    ptx::bulk_store(p.det_out + orow * rw, stg + l * rw, (uint32_t)(len * rw * 4));
+    ptx::tma_store_commit();
+  }
+  probe(p, ti, PH_STORED);
+}
+
+// RECORDS: the Detect head with compact records (epilogue_records); otherwise epilogue<NI>, which serves every other launch
+template <int NI, bool RECORDS>
 __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_kernel(const __grid_constant__ ConvK p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
@@ -439,15 +574,19 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
   float acc[NI / 2];
 #pragma unroll
   for (int i = 0; i < NI / 2; ++i) acc[i] = 0.0f;
-  int s = 0, prev_s = -1;
+  float* bt_s = bias_s + ((p.cout_pad + 32 + 31) & ~31);  // epilogue_records: the theta biases of anchor bt_nt
+  int bt_nt = -1;
+  int s = 0, prev_s = -1, ti = 0;
   uint32_t ph = 0, s_lo = ring_lo;
-  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
     const TileCoord c = decode_tile(p, t);
     uint32_t scale_d = 0u, bres_lo = res_lo;
     int kc = 0;
+    probe(p, ti, PH_TILE);
     for (int u0 = 0; u0 < n_units; u0 += group) {
       const int ng = min(group, n_units - u0);
       ptx::mbar_wait(&full_bar[s], ph);
+      if (u0 == 0) probe(p, ti, PH_FULL);
       ptx::wgmma_fence_regs(acc);
       ptx::wgmma_fence();
       uint32_t u_lo = s_lo;
@@ -488,8 +627,22 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
     __syncwarp();
     if (lane == 0) ptx::mbar_arrive(&empty_bar[prev_s]);
     prev_s = -1;
-    epilogue<NI>(p, c, acc, stg, bias_s, wg * 64 + (warp & 3) * 16, lane);
+    probe(p, ti, PH_MMA);
+    if constexpr (RECORDS) {
+      if (c.nt != bt_nt) {  // every consumer warp walks the same tiles, so all of them come here together
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * CONSUMER_WARPS) : "memory");  // no warp reads the old anchor's any more
+        const int nfix = p.det_no - 180;
+        for (int col = threadIdx.x; col < NI; col += 32 * CONSUMER_WARPS)
+          bt_s[col] = (col >= nfix && col < p.det_no) ? bias_s[c.n0 + col] : -INFINITY;
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * CONSUMER_WARPS) : "memory");
+        bt_nt = c.nt;
+      }
+      epilogue_records<NI>(p, c, acc, bt_s, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
+    } else {
+      epilogue<NI>(p, c, acc, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
+    }
   }
+  if constexpr (RECORDS) ptx::tma_store_wait_all();  // the records' bulk stores complete before the CTA exits
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -523,15 +676,24 @@ typedef void (*KernelFn)(ConvK);
 int ctas_for(int ni) { return ni <= 96 ? 2 : 1; }  // Occupancy<NI>::CTAS
 KernelFn kernel_for(int ni) {
   switch (ni) {
-    case 16: return conv_wgmma_kernel<16>;
-    case 32: return conv_wgmma_kernel<32>;
-    case 64: return conv_wgmma_kernel<64>;
-    case 96: return conv_wgmma_kernel<96>;
-    case 128: return conv_wgmma_kernel<128>;
-    case 160: return conv_wgmma_kernel<160>;
-    case 192: return conv_wgmma_kernel<192>;
-    case 224: return conv_wgmma_kernel<224>;
-    case 256: return conv_wgmma_kernel<256>;
+    case 16: return conv_wgmma_kernel<16, false>;
+    case 32: return conv_wgmma_kernel<32, false>;
+    case 64: return conv_wgmma_kernel<64, false>;
+    case 96: return conv_wgmma_kernel<96, false>;
+    case 128: return conv_wgmma_kernel<128, false>;
+    case 160: return conv_wgmma_kernel<160, false>;
+    case 192: return conv_wgmma_kernel<192, false>;
+    case 224: return conv_wgmma_kernel<224, false>;
+    case 256: return conv_wgmma_kernel<256, false>;
+    default: return nullptr;
+  }
+}
+// compact records need det_no > 180, so an N tile of at least 192 columns
+KernelFn records_kernel_for(int ni) {
+  switch (ni) {
+    case 192: return conv_wgmma_kernel<192, true>;
+    case 224: return conv_wgmma_kernel<224, true>;
+    case 256: return conv_wgmma_kernel<256, true>;
     default: return nullptr;
   }
 }
@@ -618,7 +780,10 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
   const int Hout = geom ? d->out_h : (d->Hin + 2 * d->pad_h - d->KH) / d->stride + 1;
   const int Wout = geom ? d->out_w : (d->Win + 2 * d->pad_w - d->KW) / d->stride + 1;
   const int ni = instr_n(bn);
-  o->fn = kernel_for(ni);
+  // compact records take epilogue_records when a record fits the 64-column staging row (nc <= 58)
+  const bool records = d->mode == MODE_DETECT && d->det_decode == 2 && d->det_no > 180 &&
+                       ((d->det_no - 180 + 1) + 3) / 4 * 4 <= 64 && !(d->flags & Y5OBB_CONV_DETECT_GENERIC);
+  o->fn = records ? records_kernel_for(ni) : kernel_for(ni);
   if (!o->fn) {
     delete o;
     return Y5OBB_EINVAL;
@@ -643,7 +808,8 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
   k.b_stage_bytes = (uint32_t)align_up(k.b_bytes, 1024);
   int a_rows = 0;
   size_t stage_bytes = 0;
-  const size_t bias_bytes = align_up((size_t)(cout_pad + 32) * 4, 128);  // the bias lives in shared memory behind the staging buffers
+  // the bias lives in shared memory behind the staging buffers (records: then NI floats of theta biases, see bt_s)
+  const size_t bias_bytes = align_up((size_t)(cout_pad + 32) * 4, 128) + (records ? (size_t)ni * 4 : 0);
   const size_t fixed_bytes = 1024 + (size_t)CONSUMER_WARPS * stg_bytes(ni) + bias_bytes;  // alignment slack, staging, bias
   size_t SMEM_BUDGET = 0;  // for the operand ring and the resident weights: set per CTAs-per-SM choice below
   // Row-shift mode (stride-1 convs with KH > 1): an 8 x 16 pixel tile whose A stage holds Ht + KH - 1 image
@@ -717,8 +883,8 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     delete o;
     return Y5OBB_EINVAL;
   }
-  static bool attr_set[257] = {};  // per instantiation (one per NI)
-  if (!attr_set[ni]) {
+  static bool attr_set[2][257] = {};  // per instantiation (NI, records)
+  if (!attr_set[records][ni]) {
     // all of the unified L1 / shared memory as shared memory, so that two 112 KB CTAs fit beside each other
     cudaError_t e = cudaFuncSetAttribute(o->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
     if (e == cudaSuccess)
@@ -727,7 +893,7 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
       delete o;
       return cuda_fail(e);
     }
-    attr_set[ni] = true;
+    attr_set[records][ni] = true;
   }
   auto smem_of_plan = [&]() { return k.b_res_bytes + (size_t)k.stages * stage_bytes + fixed_bytes; };
   o->smem = smem_of_plan();
@@ -895,3 +1061,19 @@ int y5obb_conv_schedule(const y5obb_conv_t* conv, int* ctas_per_sm, int* residen
 void y5obb_conv_destroy(y5obb_conv_t* conv) { delete reinterpret_cast<ConvObj*>(conv); }
 
 }  // extern "C"
+
+#ifdef Y5OBB_DETECT_PROBE
+// the probe build's stamps (see g_probe): copies them to `host` ([PROBE_CTAS][PROBE_TILES][PROBE_PHASES] int64, `bytes` long)
+// and zeroes them; returns the element count of each dimension in dims[3]
+extern "C" int y5obb_detect_probe(void* host, size_t bytes, int* dims) {
+  if (bytes < sizeof(g_probe) || !host || !dims) return Y5OBB_EINVAL;
+  cudaError_t e = cudaMemcpyFromSymbol(host, g_probe, sizeof(g_probe));
+  static long long zeros[PROBE_CTAS][PROBE_TILES][PROBE_PHASES];
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_probe, zeros, sizeof(g_probe));
+  if (e != cudaSuccess) return cuda_fail(e);
+  dims[0] = PROBE_CTAS;
+  dims[1] = PROBE_TILES;
+  dims[2] = PROBE_PHASES;
+  return Y5OBB_OK;
+}
+#endif

@@ -23,6 +23,14 @@ __device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, float a, float b, float c, float d) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_v2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
+}
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
@@ -129,6 +137,13 @@ __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* s
   asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
                "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
+}
+// plain bulk copy shared -> global (no tensor map): `bytes` a multiple of 16, both addresses 16-byte aligned.  The
+// shared-memory writes it reads must be ordered before it by fence_proxy_async (generic -> async proxy).
+__device__ __forceinline__ void bulk_store(void* gmem, const void* smem, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(reinterpret_cast<uint64_t>(gmem)),
+               "r"(smem_u32(smem)), "r"(bytes)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
