@@ -23,8 +23,8 @@ PAD_ROWS = 37           # rows of sentinel before and after the plan's region
 
 
 @functools.lru_cache(maxsize=None)
-def _model(size):
-    return calibrated_bench_model(size, nc=bench.NC, seed=0, conf=bench.CONF).to(DEV)
+def _model(size, nc=bench.NC):
+    return calibrated_bench_model(size, nc=nc, seed=0, conf=bench.CONF).to(DEV)
 
 
 def _batch(B, H, W, seed):
@@ -46,8 +46,8 @@ def _compare(a, b, what):
                              f"{a[tuple(bad[0])].item()!r} vs {b[tuple(bad[0])].item()!r}")
 
 
-def _records(size, B, H, W, seed=0):
-    m = _model(size)
+def _records(size, B, H, W, seed=0, nc=bench.NC):
+    m = _model(size, nc)
     x = _batch(B, H, W, seed)
     probe = InferenceEngine(m, B, H, W, DEV, compact_detect=True)
     rows, rec_w = probe.rows_total, probe.rec_w

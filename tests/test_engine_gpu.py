@@ -18,7 +18,7 @@ ROOT = Path(__file__).resolve().parents[1]
 DEV = "cuda:0"
 
 
-def _compare(got, ref, what):
+def _compare(got, ref, what, nc=15):
     got, ref = got.float().cpu(), ref.float().cpu()
     err = (got - ref).abs()
     tol = ref.abs() * 3e-2 + 3e-2
@@ -26,7 +26,7 @@ def _compare(got, ref, what):
     print(f"{what}: max err {err.max().item():.4g}, mean err {err.mean().item():.4g}, out-of-tol {frac_bad:.2e}")
     assert frac_bad < 1e-3, f"{what}: {frac_bad:.3e} of elements out of tolerance (max {err.max().item():.4g})"
     assert err.mean().item() < 4e-3
-    am_g, am_r = got[..., 20:].argmax(-1), ref[..., 20:].argmax(-1)
+    am_g, am_r = got[..., 5 + nc:].argmax(-1), ref[..., 5 + nc:].argmax(-1)
     assert (am_g == am_r).float().mean().item() > 0.97
 
 

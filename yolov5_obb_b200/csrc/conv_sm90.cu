@@ -325,7 +325,14 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
           }
         }
         const long long orow = (long long)c.b * p.det_rows_per_image + p.det_row_off + ((long long)a * p.Hout + h) * p.Wout + w;
-        *reinterpret_cast<float4*>(p.det_out + orow * rw + col) = make_float4(f[0], f[1], f[2], f[3]);
+        float* dst = p.det_out + orow * rw + col;
+        if (!(rw & 3)) {
+          *reinterpret_cast<float4*>(dst) = make_float4(f[0], f[1], f[2], f[3]);
+        } else {  // det_no % 4 != 0 (records are always 4-aligned): rows start 4-byte aligned and the last vector ends the row early
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (col + k < ncols) dst[k] = f[k];
+        }
       }
     }
     __syncwarp();
@@ -957,9 +964,11 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
       return Y5OBB_EINVAL;
     }
   } else {
+    // rows of rw floats: 16-byte vector stores when rw % 4 == 0 (always for records), element stores otherwise
     const int rw = d->det_decode == 2 ? k.det_rec_w : d->det_no;
-    if (!d->det_out || d->det_no % 4 || (d->det_decode == 2 && d->det_no <= 180) ||
-        (reinterpret_cast<uintptr_t>(d->det_out + (size_t)d->det_row_off * rw) & 15)) {
+    const uintptr_t align = rw % 4 ? 3 : 15;
+    if (!d->det_out || (d->det_decode == 2 && d->det_no <= 180) ||
+        (reinterpret_cast<uintptr_t>(d->det_out + (size_t)d->det_row_off * rw) & align)) {
       delete o;
       return Y5OBB_EINVAL;
     }

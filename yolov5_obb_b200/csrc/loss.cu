@@ -415,20 +415,22 @@ __global__ void k_head_rows(LossK L, HeadK hk) {
   const __nv_bfloat16* w = h.w + (long long)r.a * L.no * h.C;
   const float* bias = h.bias + r.a * L.no;
   float* out = L.head_rows + (long long)L.rank[q] * L.no;
-  for (int j0 = 0; j0 < L.no; j0 += 4) {  // no % 4 == 0 (fill)
+  for (int j0 = 0; j0 < L.no; j0 += 4) {  // the last group of a row whose no % 4 != 0 has fewer than 4 logits
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     for (int c8 = lane; c8 < C8; c8 += 32) {
       const uint4 v = __ldg(reinterpret_cast<const uint4*>(f + c8 * 8));
 #pragma unroll
       for (int k = 0; k < 4; ++k)
-        acc[k] = dot8(v, __ldg(reinterpret_cast<const uint4*>(w + (long long)(j0 + k) * h.C + c8 * 8)), acc[k]);
+        if (j0 + k < L.no)
+          acc[k] = dot8(v, __ldg(reinterpret_cast<const uint4*>(w + (long long)(j0 + k) * h.C + c8 * 8)), acc[k]);
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
     }
-    if (lane < 4) out[j0 + lane] = bias[j0 + lane] + (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]);
+    if (lane < 4 && j0 + lane < L.no)
+      out[j0 + lane] = bias[j0 + lane] + (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]);
   }
 }
 
@@ -472,24 +474,32 @@ __global__ void __launch_bounds__(256) k_final(LossK L, float* loss, float* item
   }
 }
 
-// dense gradient: every cell row is written exactly once here (zeros + obj channel)
+// dense gradient: every element of the level is written exactly once here (zeros + obj channel).  The level's cells * no
+// floats are walked flat, as float4s (the buffer is 16-byte aligned) and then a scalar tail of (cells * no) % 4; when
+// no % 4 != 0 a vector may span the end of one cell's row and the start of the next.
 __global__ void k_bwd_obj(LossK L, int lvl, const float* __restrict__ gloss) {
   const long long cells = L.cell_off[lvl + 1] - L.cell_off[lvl];
-  const long long vec_per_cell = L.no / 4;
-  const long long total = cells * vec_per_cell;
+  const long long n = cells * L.no, nvec = n / 4;
   const float g = gloss[0] * (float)L.B * L.hyp_obj * L.balance[lvl] / (float)cells;
-  float4* out = reinterpret_cast<float4*>(L.grad[lvl]);
+  auto obj_grad = [&](long long cell) {
+    const float x = L.p[lvl][cell * L.no + 4];
+    const int w = L.winner[L.cell_off[lvl] + cell];
+    const float t = w >= 0 ? fmaxf(L.row_iou[w], 0.f) : 0.f;
+    return g * bce_logits_grad(x, t, L.obj_pw);
+  };
+  float* out = L.grad[lvl];
+  const long long total = nvec + (n & 3);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long cell = i / vec_per_cell;
-    const int v = (int)(i - cell * vec_per_cell);
-    float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (v == 1) {  // channels 4..7: obj is channel 4
-      const float x = L.p[lvl][cell * L.no + 4];
-      const int w = L.winner[L.cell_off[lvl] + cell];
-      const float t = w >= 0 ? fmaxf(L.row_iou[w], 0.f) : 0.f;
-      o.x = g * bce_logits_grad(x, t, L.obj_pw);
+    if (i < nvec) {
+      const long long e = 4 * i, cell = e / L.no;
+      const int ch = (int)(e - cell * L.no);  // channel of the vector's first element
+      // obj (channel 4 of `cell`) is element 4 - ch when ch is 1..4; the next cell's channel 4 lies no >= 185 floats further
+      const float v = (ch >= 1 && ch <= 4) ? obj_grad(cell) : 0.f;
+      reinterpret_cast<float4*>(out)[i] = make_float4(ch == 4 ? v : 0.f, ch == 3 ? v : 0.f, ch == 2 ? v : 0.f, ch == 1 ? v : 0.f);
+    } else {
+      const long long e = 4 * nvec + (i - nvec), cell = e / L.no;
+      out[e] = e - cell * L.no == 4 ? obj_grad(cell) : 0.f;
     }
-    out[i] = o;
   }
 }
 
@@ -525,7 +535,7 @@ __global__ void k_bwd_rows(LossK L, const float* __restrict__ gloss) {
 
 int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* need, bool head = false) {
   if (!d || d->nl < 1 || d->nl > NL || d->B < 1 || d->na < 1 || d->na > 3 || d->nt < 0) return Y5OBB_EINVAL;
-  if (d->no != d->nc + 5 + 180 || d->no % 4) return Y5OBB_EINVAL;
+  if (d->no != d->nc + 5 + 180) return Y5OBB_EINVAL;
   if (d->tcols != 7 && d->tcols != 8 && d->tcols < 7 + 180) return Y5OBB_EINVAL;
   memset(&L, 0, sizeof(L));
   L.csl_mode = d->tcols == 7 ? 2 : (d->tcols == 8 ? 1 : 0);
@@ -736,7 +746,7 @@ int y5obb_loss_backward(const y5obb_loss_desc* d, const float* grad_loss, void* 
   const int real_cand = L.ncand;
   if (L.ncand == 0) L.ncand = 1;
   for (int lvl = 0; lvl < L.nl; ++lvl) {
-    const long long total = (L.cell_off[lvl + 1] - L.cell_off[lvl]) * (L.no / 4);
+    const long long total = (L.cell_off[lvl + 1] - L.cell_off[lvl]) * L.no / 4 + 3;  // >= k_bwd_obj's float4s + tail
     const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 32);
     k_bwd_obj<<<grid, 256, 0, st>>>(L, lvl, grad_loss);
     Y5_LAUNCH_CHECK();

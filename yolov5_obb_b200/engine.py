@@ -24,6 +24,7 @@ import torch
 
 from . import _lib
 from .conv import Conv as ConvOp, Slice, pack_weights, MODE_DETECT
+from .general import require_nc
 from .layout import _is, route, shapes, sources, stem_weight, stem_window
 from . import yolo as Y
 
@@ -56,6 +57,7 @@ class InferenceEngine:
         if device.type != "cuda":
             raise RuntimeError("InferenceEngine needs a CUDA device (sm_90a); there is no CPU path")
         det = model.model[-1]
+        require_nc(det.nc, "InferenceEngine")
         smax = int(max(model.stride))
         if H % smax or W % smax:
             raise RuntimeError(f"image size {H}x{W} must be a multiple of the max stride {smax}")
@@ -325,6 +327,7 @@ class TTAPlan:
         if device.type != "cuda":
             raise RuntimeError("TTAPlan needs a CUDA device (sm_90a); there is no CPU path")
         det = model.model[-1]
+        require_nc(det.nc, "TTAPlan")
         self.branches, self.rows_total = tta_geometry(H, W, int(max(model.stride)), det.nl, det.na,
                                                       [int(s) for s in det.stride])
         self.device, self.B, self.H, self.W = device, B, H, W

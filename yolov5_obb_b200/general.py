@@ -10,6 +10,14 @@ from . import _lib
 
 MAX_WH = 4096     # general.py:793
 MAX_NMS = 30000   # general.py:794
+NC_MAX = 64       # class counts 1..64: NMS keeps the allowed classes in one 64-bit mask; Detect's no = nc + 185 <= 249 fits a
+                  # 256-column N tile
+
+
+def require_nc(nc: int, what: str) -> None:
+    """Refuses a class count outside 1..NC_MAX, naming `what` and the range."""
+    if not 1 <= int(nc) <= NC_MAX:
+        raise RuntimeError(f"{what}: nc={nc} is not supported; the class count must be 1..{NC_MAX}")
 
 
 class DetectRecords:
@@ -43,8 +51,7 @@ def non_max_suppression_obb(prediction: torch.Tensor, conf_thres: float = 0.25, 
     assert 0 <= iou_thres <= 1, f'Invalid IoU {iou_thres}, valid values are between 0.0 and 1.0'
     if labels:
         raise RuntimeError("apriori `labels` (autolabelling) are not part of the hot path")
-    if nc < 1 or nc > 64:
-        raise RuntimeError(f"nc={nc} unsupported (1..64)")
+    require_nc(nc, "non_max_suppression_obb")
     B, A, no = prediction.shape
     if compact:
         no = nc + 185

@@ -13,6 +13,7 @@ from ctypes import c_void_p, c_int, c_int64, c_float
 import torch
 
 from . import _lib
+from .general import require_nc
 
 MAX_LEVELS = 4  # Y5OBB_LOSS_MAX_LEVELS (include/y5obb.h): the P3-P6 Detect of models/hub/yolov5*6.yaml
 
@@ -98,6 +99,7 @@ class ComputeLoss:
         self.gr, self.hyp, self.autobalance = 1.0, h, autobalance
         for k in "na", "nc", "nl", "anchors":
             setattr(self, k, getattr(det, k))
+        require_nc(self.nc, "ComputeLoss")
         if self.nl not in (3, MAX_LEVELS) or self.na > 3:
             raise RuntimeError(f"the loss takes the 3-level Detect of yolov5{{n,s,m,l,x}}.yaml or the {MAX_LEVELS}-level one of "
                                f"models/hub/yolov5{{n,s,m,l,x}}6.yaml, with at most 3 anchors per level; this one has "

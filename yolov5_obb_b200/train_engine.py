@@ -13,6 +13,7 @@ import torch
 
 from . import _lib
 from .conv import Conv as ConvOp, Slice, pack_weights, MODE_DETECT
+from .general import require_nc
 from .layout import _is, route, shapes, sources, stem_weight, stem_window
 
 
@@ -124,6 +125,7 @@ class TrainEngine:
         if device.type != "cuda":
             raise RuntimeError("TrainEngine needs a CUDA device (sm_90a); there is no CPU path")
         det = model.model[-1]
+        require_nc(det.nc, "TrainEngine")
         smax = int(max(model.stride))
         if H % smax or W % smax:
             raise RuntimeError(f"image size {H}x{W} must be a multiple of the max stride {smax}")
