@@ -349,14 +349,16 @@ int y5obb_detect_grad_pack(const float* g, void* out_nhwc, int B, int na, int H,
  * fp32 nn.Conv2d parameters [Cout][Cin][KH][KW] -> the bf16 operand layouts the conv kernel's TMA descriptors point at,
  * all layers in one launch.  dst is [taps][rows_pad][cols_pad] bf16 (DETECT_BIAS: fp32 [cols_pad]):
  *   FWD           rows = Cout, cols = Cin                         (y5obb_conv_run forward)
- *   DGRAD         rows = Cin,  cols = Cout, taps flipped          (data gradient = conv with transposed weights)
+ *   DGRAD         rows = Cin,  cols = Cout, taps flipped          (data gradient = conv with transposed weights);
+ *                 group_pad > 0: rows = the input-channel window [group_real, group_real + group_pad) of Cin only (the
+ *                 gradient of part of a Concat); group_real = group_pad = 0: every input channel
  *   STEM          the 6x6/s2 stem as a 3x1 conv over the 48-channel space-to-depth window (KH=6,KW=6 in; 3 taps out)
  *   DETECT        rows grouped per anchor: group_real real rows padded to group_pad (models/yolo.py:49-65)
  *   DETECT_DGRAD  rows = Cin, cols grouped per anchor
  *   DETECT_BIAS   fp32 bias, grouped per anchor
  *   DGRAD_S2      data gradient of a 3x3 / stride-2 / pad-1 conv for output-pixel parity (ph, pw) = (group_real >> 1,
  *                 group_real & 1): rows = Cin, cols = Cout, (ph ? 2 : 1) x (pw ? 2 : 1) taps; tap t along an axis of parity 1
- *                 is source tap (t == 0 ? 2 : 0), along an axis of parity 0 source tap 1 */
+ *                 is source tap (t == 0 ? 2 : 0), along an axis of parity 0 source tap 1; group_pad must be 0 (no window) */
 enum { Y5OBB_PACK_FWD = 0, Y5OBB_PACK_DGRAD = 1, Y5OBB_PACK_STEM = 2, Y5OBB_PACK_DETECT = 3, Y5OBB_PACK_DETECT_DGRAD = 4,
        Y5OBB_PACK_DETECT_BIAS = 5, Y5OBB_PACK_DGRAD_S2 = 6 };
 typedef struct y5obb_pack_plan y5obb_pack_plan_t;

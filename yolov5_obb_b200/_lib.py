@@ -170,6 +170,8 @@ def workspace(nbytes: int, device, tag: str = "default") -> torch.Tensor:
     key = (torch.device(device).index or 0, tag)
     buf = _WS.get(key)
     if buf is None or buf.numel() < nbytes:
+        _WS.pop(key, None)   # the smaller buffer goes first: growing never holds both
+        del buf
         buf = torch.empty(int(nbytes * 1.25) + 4096, dtype=torch.uint8, device=device)
         _WS[key] = buf
     return buf

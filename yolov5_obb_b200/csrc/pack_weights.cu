@@ -35,9 +35,10 @@ __device__ __forceinline__ float pack_value(const PackEntryK& e, int tap, int ro
       if (row >= e.Cout || col >= e.Cin) return 0.f;
       return e.src[(((long long)row * e.Cin + col) * e.KH + kh) * e.KW + kw];
     }
-    case Y5OBB_PACK_DGRAD: {  // the dgrad conv has Cout' = Cin, Cin' = Cout: row = ci, col = co, taps flipped
-      if (row >= e.Cin || col >= e.Cout) return 0.f;
-      return e.src[(((long long)col * e.Cin + row) * e.KH + (e.KH - 1 - kh)) * e.KW + (e.KW - 1 - kw)];
+    case Y5OBB_PACK_DGRAD: {  // the dgrad conv has Cout' = Cin, Cin' = Cout: row = ci - c0, col = co, taps flipped
+      // (a channel window [c0, c0 + n) = [g_real, g_real + g_pad) of Cin when g_pad > 0: the gradient of those inputs only)
+      if (row >= (e.g_pad ? e.g_pad : e.Cin) || col >= e.Cout) return 0.f;
+      return e.src[(((long long)col * e.Cin + (e.g_real + row)) * e.KH + (e.KH - 1 - kh)) * e.KW + (e.KW - 1 - kw)];
     }
     case Y5OBB_PACK_DGRAD_S2: {  // tap = th * KW' + tw of the parity class (ph, pw) = (g_real >> 1, g_real & 1)
       if (row >= e.Cin || col >= e.Cout) return 0.f;
@@ -112,7 +113,12 @@ int y5obb_pack_plan_create(const y5obb_pack_entry* entries, int n, y5obb_pack_pl
     if (!e.src || !e.dst || e.Cout <= 0 || e.Cin <= 0 || e.KH <= 0 || e.KW <= 0 || e.rows_pad <= 0 || e.cols_pad <= 0 ||
         e.kind < Y5OBB_PACK_FWD || e.kind > Y5OBB_PACK_DGRAD_S2)
       return Y5OBB_EINVAL;
-    if (e.kind == Y5OBB_PACK_DGRAD_S2 && (e.KH != 3 || e.KW != 3 || e.group_real < 0 || e.group_real > 3)) return Y5OBB_EINVAL;
+    if (e.kind == Y5OBB_PACK_DGRAD && (e.group_pad < 0 || e.group_real < 0 || e.group_real + e.group_pad > e.Cin ||
+                                       (e.group_pad == 0 && e.group_real != 0)))
+      return Y5OBB_EINVAL;
+    // the stride-2 phases take no channel window: group_pad must stay 0
+    if (e.kind == Y5OBB_PACK_DGRAD_S2 && (e.KH != 3 || e.KW != 3 || e.group_real < 0 || e.group_real > 3 || e.group_pad != 0))
+      return Y5OBB_EINVAL;
     const bool grouped = e.kind >= Y5OBB_PACK_DETECT && e.kind <= Y5OBB_PACK_DETECT_BIAS;
     if (grouped && (e.group_real <= 0 || e.group_pad < e.group_real)) return Y5OBB_EINVAL;
     PackEntryK& k = h[(size_t)i];

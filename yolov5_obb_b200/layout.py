@@ -116,3 +116,42 @@ def stem_window(x_s2d: torch.Tensor) -> WindowView:
     B, h, wp, c = x_s2d.shape
     return WindowView(buf=x_s2d, ptr=x_s2d.data_ptr(), pix_stride=c, row_stride=wp * c, img_stride=h * wp * c, B=B, H=h,
                       W=wp - 2, C=3 * c, hbm_c=c)
+
+
+# ---- which gradients a backward pass computes when some parameters are frozen (train.py --freeze)
+def needs_grad(nodes, owns) -> set:
+    """The liveness rule: the gradient of a node's output is needed iff the node, or a node upstream of it, owns a
+    trainable parameter.  nodes: (node, the nodes it reads) in forward order; owns(node) -> bool."""
+    need = set()
+    for n, srcs in nodes:
+        if owns(n) or any(s in need for s in srcs):
+            need.add(n)
+    return need
+
+
+def merge_windows(ranges) -> List[Tuple[int, int]]:
+    """Channel ranges [(lo, hi)], sorted, with touching or overlapping ranges joined."""
+    out: List[Tuple[int, int]] = []
+    for lo, hi in sorted(ranges):
+        if out and lo <= out[-1][1]:
+            out[-1] = (out[-1][0], max(out[-1][1], hi))
+        else:
+            out.append((lo, hi))
+    return out
+
+
+def grad_liveness(layers, ch, trainable):
+    """The liveness rule over the model graph.  trainable(m) -> whether layer m owns a trainable parameter.
+    Returns (needed, windows): the indices of the layers whose output gradient is needed, and per needed Concat the channel
+    windows of its output whose gradient is needed (the slices of its inputs that are in `needed`)."""
+    need = needs_grad([(m.i, sources(m) if m.i else []) for m in layers], lambda i: trainable(layers[i]))
+    windows = {}
+    for m in layers:
+        if _is(m, "Concat") and m.i in need:
+            off, w = 0, []
+            for s in sources(m):
+                if s in need:
+                    w.append((off, off + ch[s]))
+                off += ch[s]
+            windows[m.i] = merge_windows(w)
+    return need, windows

@@ -10,6 +10,13 @@ Gradient buffers mirror the activation buffers; whether a contribution overwrite
 statically when the plan is built (first writer of a channel range overwrites).
 Parameter gradients land in views of ONE flat fp32 buffer owned by the plan (run() returns it); the autograd
 Function in yolo.py hands them to autograd, which accumulates into `.grad` (so GradScaler / DDP hooks see them).
+
+Frozen parameters (train.py --freeze, `requires_grad = False`): a plan is built for one set of trainable flags and
+computes only what those need (layout.needs_grad).  A Conv's BatchNorm backward runs iff its output gradient is needed, its
+wgrad iff its weight is trainable, a dgrad / upsample / pool backward iff the producer of what it writes needs a gradient;
+a dgrad into a Concat whose inputs are partly live computes only the live channel window (a conv whose output is that
+window of the gradient buffer, with the matching window of the weight packed).  The launches that remain are the full
+plan's, in its order, with its descriptors.
 """
 import os
 from typing import Dict, List, Optional
@@ -18,7 +25,7 @@ import torch
 
 from . import _lib
 from .conv import Conv as ConvOp, Slice, pack_weights, tiling, MODE_DETECT
-from .layout import stem_grad
+from .layout import merge_windows, needs_grad, stem_grad
 from .train_engine import _PoolLayer, flat_layout
 from .train_ops import Wgrad
 
@@ -59,7 +66,8 @@ class _Written:
 
 
 class BackwardPlan:
-    def __init__(self, eng):
+    def __init__(self, eng, trainable=None):
+        """trainable: requires_grad of every parameter, in model.parameters() order (None: all of them)."""
         self.eng = eng
         dev = eng.device
         B = eng.B
@@ -84,7 +92,10 @@ class BackwardPlan:
         written = _Written()
         det = eng.model.model[-1]
 
-        # activation-sized buffers come from the engine's allocator (its arena when one is reserved, train_engine.TrainArena)
+        # activation-sized buffers come from the engine's allocator (its arena when one is reserved, train_engine.TrainArena);
+        # every backward plan of an engine (one per set of trainable flags) starts where the forward's buffers end: in an arena
+        # they share those bytes, as plans of different shapes do, since only one of them runs at a time
+        eng._carver.off = eng.fwd_bytes
         carve = eng._carver.take
 
         def gslice(s: Slice) -> Slice:
@@ -118,9 +129,18 @@ class BackwardPlan:
             self.flat = torch.zeros(n, dtype=torch.float32, device=dev)
         self.pgrad: Dict[torch.nn.Parameter, torch.Tensor] = {
             p: self.flat[o:o + p.numel()].view(p.shape) for p, o in zip(self.params, self.offsets)}
+        self.trainable = tuple(True for _ in self.params) if trainable is None else tuple(bool(t) for t in trainable)
+        if len(self.trainable) != len(self.params):
+            raise ValueError(f"trainable has {len(self.trainable)} flags for {len(self.params)} parameters")
+        self._live_out, self.live_windows = self._liveness(eng)
 
         def grad_of(p: torch.nn.Parameter) -> torch.Tensor:
             return self.pgrad[p]
+
+        flag = dict(zip(map(id, self.params), self.trainable))
+
+        def trains(p: torch.nn.Parameter) -> bool:
+            return flag[id(p)]
 
         self._grad_of = grad_of
 
@@ -141,38 +161,46 @@ class BackwardPlan:
             cv = eng.det_convs[l]
             xin: Slice = cv._keep[0]
             mi = det.m[l]
+            if ("det", l) not in self._live_out:
+                continue
             H, W, Cin = xin.H, xin.W, xin.C
             bk, bn, cin_pad, cout_pad, nt = tiling(Cin, det.na * det.no, MODE_DETECT, det.no)
             dzd = bf(B, H, W, det.na * bn)
-            s1, s2 = f32(det.na * bn), f32(det.na * bn)
-            part = dict(l=l, dzd=dzd, s1=s1, bn=bn, Cin=Cin, mi=mi)
+            part = dict(l=l, dzd=dzd, s1=None, bn=bn, Cin=Cin, mi=mi)
             self.det_parts.append(part)
 
             def pack_step(st, l=l, dzd=dzd, H=H, W=W, bn=bn):
                 g = self.det_grads_in[l]
                 _lib.check(L.y5obb_detect_grad_pack(g.data_ptr(), dzd.data_ptr(), B, det.na, H, W, det.no, bn, st), "detect_grad_pack")
             add("detect_pack", pack_step)
-            # bias gradient = per-channel sums of dz
-            add("detect_bias", lambda st, dzd=dzd, s1=s1, s2=s2, n=B * H * W, C=det.na * bn:
-                              _lib.check(L.y5obb_bn_stats(dzd.data_ptr(), C, n, C, s1.data_ptr(), s2.data_ptr(), eng.scratch.data_ptr(),
-                                                          eng.scratch.numel(), st), "detect bias grad"))
-            wg = Wgrad(dzd.data_ptr(), det.na * bn, xin.ptr, xin.pix_stride, grad_of(mi.weight), B, det.na * bn, H, W, Cin, H, W,
-                       1, 1, 0, keep=(dzd, xin.buf, self.flat), param_layout=True, co_group=(det.no, bn))
-            self.keep.append(wg)
-            part["wgrad"] = wg
-            self.flops += 2.0 * B * H * W * det.na * bn * Cin
-            add("wgrad", lambda st, wg=wg: wg.run(st))
-            # dgrad: gx (+)= dz @ W  (1x1): weights [Cout'=Cin][Cin'=na*bn]
-            wT = torch.zeros((Cin, det.na * bn, 1, 1), device=dev)
-            part["wT"] = wT
-            op, wp = add_dgrad(Slice.full(dzd), wT, 1, 0, gslice(xin), "detect dgrad")
-            part["dgrad_wp"] = wp
-            part["dgrad_ops"] = [op]
-            self.keep.append(op)
+            if trains(mi.bias):  # bias gradient = per-channel sums of dz
+                s1, s2 = f32(det.na * bn), f32(det.na * bn)
+                part["s1"] = s1
+                add("detect_bias", lambda st, dzd=dzd, s1=s1, s2=s2, n=B * H * W, C=det.na * bn:
+                                  _lib.check(L.y5obb_bn_stats(dzd.data_ptr(), C, n, C, s1.data_ptr(), s2.data_ptr(),
+                                                              eng.scratch.data_ptr(), eng.scratch.numel(), st), "detect bias grad"))
+            if trains(mi.weight):
+                wg = Wgrad(dzd.data_ptr(), det.na * bn, xin.ptr, xin.pix_stride, grad_of(mi.weight), B, det.na * bn, H, W, Cin,
+                           H, W, 1, 1, 0, keep=(dzd, xin.buf, self.flat), param_layout=True, co_group=(det.no, bn))
+                self.keep.append(wg)
+                part["wgrad"] = wg
+                self.flops += 2.0 * B * H * W * det.na * bn * Cin
+                add("wgrad", lambda st, wg=wg: wg.run(st))
+            if self.live_windows(xin):  # (a Detect input is one layer's output: live as a whole or not at all)
+                # dgrad: gx (+)= dz @ W  (1x1): weights [Cout'=Cin][Cin'=na*bn]
+                wT = torch.zeros((Cin, det.na * bn, 1, 1), device=dev)
+                part["wT"] = wT
+                op, wp = add_dgrad(Slice.full(dzd), wT, 1, 0, gslice(xin), "detect dgrad")
+                part["dgrad_wp"] = wp
+                part["dgrad_ops"] = [op]
+                self.keep.append(op)
 
         # ---------------- conv layers, reverse ----------------
         self.conv_parts = []
-        for lay in reversed(eng.layers):
+        for li in reversed(range(len(eng.layers))):
+            lay = eng.layers[li]
+            if li not in self._live_out:    # no trainable parameter at or upstream of this layer
+                continue
             if isinstance(lay, _PoolLayer):
                 cat4, hh, ww, c_ = lay.cat4, lay.h, lay.w, lay.c
                 gc = gslice(Slice.full(cat4))
@@ -212,7 +240,7 @@ class BackwardPlan:
             dz = bf(B, Hh, Ww, Cout)
             s1, s2 = f32(Cout), f32(Cout)
             gres, gacc = None, 0
-            if lay.res is not None:
+            if lay.res is not None and self.live_windows(lay.res):
                 gres = gslice(lay.res)
                 gacc = int(written.contribute(gres))
             part = dict(lay=lay, dz=dz)
@@ -231,29 +259,44 @@ class BackwardPlan:
 
             # ---- wgrad (straight from the NHWC buffers)
             x = lay.x
-            if lay.stem:  # the forward's window view: a 3x1 conv over 48-channel windows (3 horizontal taps x 16 s2d channels)
-                dw = f32(3 * Cout * x.C)   # gradient over the space-to-depth form, re-mapped to [Cout,3,6,6] at the end of run()
-                part["stem_dw"] = dw
-                add("zero", lambda st, dw=dw: dw.zero_())
-                wg = Wgrad(dz.data_ptr(), Cout, x.ptr, x.pix_stride, dw, B, Cout, Hh, Ww, x.C, x.H, x.W, (3, 1), 1, (1, 0),
-                           keep=(dz, x.buf), x_strides=(x.row_stride, x.img_stride))
-                ntap = 3
-            else:
-                wg = Wgrad(dz.data_ptr(), Cout, x.ptr, x.pix_stride, grad_of(conv.weight), B, Cout, Hh, Ww, x.C, x.H, x.W, k, s, p,
-                           keep=(dz, x.buf, self.flat), param_layout=True)
-                ntap = k * k
-            self.keep.append(wg)
-            part["wgrad"] = wg
-            self.flops += 2.0 * npix * Cout * x.C * ntap
-            add("wgrad", lambda st, wg=wg: wg.run(st))
+            if trains(conv.weight):
+                if lay.stem:  # the forward's window view: a 3x1 conv over 48-channel windows (3 horizontal taps x 16 s2d channels)
+                    dw = f32(3 * Cout * x.C)   # gradient over the space-to-depth form, re-mapped to [Cout,3,6,6] at the end of run()
+                    part["stem_dw"] = dw
+                    add("zero", lambda st, dw=dw: dw.zero_())
+                    wg = Wgrad(dz.data_ptr(), Cout, x.ptr, x.pix_stride, dw, B, Cout, Hh, Ww, x.C, x.H, x.W, (3, 1), 1, (1, 0),
+                               keep=(dz, x.buf), x_strides=(x.row_stride, x.img_stride))
+                    ntap = 3
+                else:
+                    wg = Wgrad(dz.data_ptr(), Cout, x.ptr, x.pix_stride, grad_of(conv.weight), B, Cout, Hh, Ww, x.C, x.H, x.W, k, s,
+                               p, keep=(dz, x.buf, self.flat), param_layout=True)
+                    ntap = k * k
+                self.keep.append(wg)
+                part["wgrad"] = wg
+                self.flops += 2.0 * npix * Cout * x.C * ntap
+                add("wgrad", lambda st, wg=wg: wg.run(st))
 
-            # ---- dgrad
-            if not lay.stem:
+            # ---- dgrad, of the input channels whose producer needs a gradient
+            win = [] if lay.stem else self.live_windows(x)
+            if win:
                 gx = gslice(x)
-                w_d = torch.zeros((x.C, Cout, k, k), device=dev)  # filled by refresh()
-                part["w_d"] = w_d
                 part["dgrad_ops"] = []  # the conv launches that produce gx, in launch order
-                if s == 1:
+                if win != [(x.c_off, x.c_off + x.C)]:
+                    # part of a Concat (the head C3s' cv1 / cv2 under a frozen backbone): one dgrad conv per live window,
+                    # writing that window of the gradient buffer, with the matching input channels of the weight packed
+                    if s != 1:
+                        raise RuntimeError(f"the data gradient of part of the input channels of a stride-{s} conv is not "
+                                           "planned (a channel window is planned for stride 1)")
+                    part["dgrad_win"] = []
+                    for lo, hi in win:
+                        w_d = torch.zeros((hi - lo, Cout, k, k), device=dev)  # filled by refresh()
+                        op, wp = add_dgrad(Slice.full(dz), w_d, k, k - 1 - p, Slice(gx.buf, lo, hi - lo), "dgrad window")
+                        part["dgrad_win"].append((lo - x.c_off, hi - lo, wp))
+                        part["dgrad_ops"].append(op)
+                        self.keep.append(op)
+                elif s == 1:
+                    w_d = torch.zeros((x.C, Cout, k, k), device=dev)  # filled by refresh()
+                    part["w_d"] = w_d
                     op, wp = add_dgrad(Slice.full(dz), w_d, k, k - 1 - p, gx, "dgrad")
                     part["dgrad_wp"] = wp
                     part["dgrad_ops"].append(op)
@@ -280,16 +323,54 @@ class BackwardPlan:
                             part["dgrad_s2"].append((ph * 2 + pw, wp))
                             part["dgrad_ops"].append(op)
                             self.keep.append(op)
+        self.nbytes = eng._carver.off - eng.fwd_bytes   # the activation-sized buffers it carved (gradients, dz, scratch)
         self.refresh()
 
     # ------------------------------------------------------------------------------------------
+    def _liveness(self, eng):
+        """layout.needs_grad over the plan's own nodes (eng.layers by index, Detect level l as ("det", l); a node reads the
+        producers of the channel ranges of its input and residual) -> (live, windows): the nodes whose output gradient
+        this plan computes, and windows(s) -> the channel ranges [lo, hi) of Slice s whose producer is live, merged."""
+        flag = dict(zip(map(id, self.params), self.trainable))
+        prod = {}   # activation buffer -> [(lo, hi, node)] of the channel ranges the forward writes into it
+
+        def producers(s):
+            lo, hi = s.c_off, s.c_off + s.C
+            return [(a, b, n) for a, b, n in prod.get(s.buf.data_ptr(), ()) if a < hi and lo < b]
+
+        nodes, owns = [], {}
+        for i, lay in enumerate(eng.layers):
+            if isinstance(lay, _PoolLayer):
+                ins, outs, params = [Slice(lay.cat4, 0, lay.c)], [Slice(lay.cat4, lay.c, 3 * lay.c)], ()
+            else:
+                ins = ([] if lay.stem else [lay.x]) + ([lay.res] if lay.res is not None else [])
+                outs = [lay.y] + ([lay.y2x] if lay.y2x is not None else [])
+                params = (lay.mod.conv.weight, lay.mod.bn.weight, lay.mod.bn.bias)
+            nodes.append((i, [n for s in ins for _, _, n in producers(s)]))
+            owns[i] = any(flag[id(p)] for p in params)
+            for o in outs:
+                prod.setdefault(o.buf.data_ptr(), []).append((o.c_off, o.c_off + o.C, i))
+        det = eng.model.model[-1]
+        for l in range(det.nl):
+            nodes.append((("det", l), [n for _, _, n in producers(eng.det_convs[l]._keep[0])]))
+            owns[("det", l)] = flag[id(det.m[l].weight)] or flag[id(det.m[l].bias)]
+        live = needs_grad(nodes, owns.__getitem__)
+
+        def windows(s):
+            lo, hi = s.c_off, s.c_off + s.C
+            return merge_windows((max(a, lo), min(b, hi)) for a, b, n in producers(s) if n in live)
+        return live, windows
+
     def pack_entries(self):
         """(kind, fp32 parameter, packed bf16 buffer, group_real, group_pad) of every data-gradient weight buffer."""
         from .train_ops import PACK_DGRAD, PACK_DETECT_DGRAD, PACK_DGRAD_S2
         det = self.eng.model.model[-1]
-        ent = [(PACK_DETECT_DGRAD, part["mi"].weight.data, part["dgrad_wp"], det.no, part["bn"]) for part in self.det_parts]
+        ent = [(PACK_DETECT_DGRAD, part["mi"].weight.data, part["dgrad_wp"], det.no, part["bn"]) for part in self.det_parts
+               if "dgrad_wp" in part]
         ent += [(PACK_DGRAD, part["lay"].mod.conv.weight.data, part["dgrad_wp"], 0, 0) for part in self.conv_parts
                 if "dgrad_wp" in part]
+        ent += [(PACK_DGRAD, part["lay"].mod.conv.weight.data, wp, c0, n) for part in self.conv_parts
+                for c0, n, wp in part.get("dgrad_win", ())]
         for part in self.conv_parts:
             for phase, wp in part.get("dgrad_s2", ()):
                 ent.append((PACK_DGRAD_S2, part["lay"].mod.conv.weight.data, wp, phase, 0))
@@ -298,7 +379,9 @@ class BackwardPlan:
     def refresh(self):
         """Pack the data-gradient weights (W transposed, taps flipped) from the current parameters."""
         from .train_ops import PackPlan
-        PackPlan(self.pack_entries(), self.eng.device).run()
+        ent = self.pack_entries()
+        if ent:   # (none when every data gradient is pruned)
+            PackPlan(ent, self.eng.device).run()
 
     def run(self, grads: List[torch.Tensor]):
         """grads: dLoss/dp for the 3 Detect outputs (fp32, same shapes as TrainEngine.det_out)."""
@@ -366,7 +449,8 @@ class BackwardPlan:
             # ---- the few gradients that need a re-mapping (tiny tensors)
             for part in self.det_parts:
                 mi, bn = part["mi"], part["bn"]
-                self.pgrad[mi.bias].copy_(part["s1"].view(det.na, bn)[:, :det.no].reshape(-1))
+                if part["s1"] is not None:
+                    self.pgrad[mi.bias].copy_(part["s1"].view(det.na, bn)[:, :det.no].reshape(-1))
             for part in self.conv_parts:
                 if "stem_dw" in part:
                     stem_grad(part["stem_dw"], self.pgrad[part["lay"].mod.conv.weight])

@@ -220,8 +220,10 @@ class TrainEngine:
             self.det_out.append(o)
             self.det_convs.append(cv)
         self.out_slices = out
+        self.fwd_bytes = self._carver.off   # where the backward plans' buffers start (train_backward.BackwardPlan)
         self.conv_layers = [lay for lay in self.layers if isinstance(lay, _BNLayer)]
         self._bwd, self._pack, self._pack_has_bwd = None, None, False
+        self._bwds = {}   # requires_grad flags of model.parameters() -> the BackwardPlan for them; _bwd: the last one run
         self.prof = None  # set to {} to collect per-kernel-kind device times (ms) during forward()
         import os
         self.use_graph = os.environ.get("Y5OBB_NO_GRAPH", "0") != "1"
@@ -356,15 +358,25 @@ class TrainEngine:
                 self.prof.setdefault(tag, []).append(e0.elapsed_time(e1))
         return self.det_out
 
-    def backward(self, grads):
+    def backward(self, grads, trainable=None):
         """grads: dLoss/d(det_out[l]) for the three levels -> the BackwardPlan, whose .flat holds every parameter
-        gradient (fp32, model.parameters() order, see train_backward.py)."""
-        if self._bwd is None:
+        gradient (fp32, model.parameters() order, see train_backward.py).  trainable: requires_grad of every parameter in
+        that order (None: the model's current flags).  One plan is kept per set of flags, each with its own graph: frozen
+        layers (train.py --freeze) cost no launch, and unfreezing builds the full plan."""
+        if trainable is None:
+            trainable = [p.requires_grad for p in self.model.parameters()]
+        key = tuple(bool(t) for t in trainable)
+        plan = self._bwds.get(key)
+        if plan is None:
             from .train_backward import BackwardPlan
             mem0 = torch.cuda.memory_allocated(self.device)
-            self._bwd = BackwardPlan(self)     # packs its data-gradient weights from the current parameters
+            plan = self._bwds[key] = BackwardPlan(self, key)   # packs its data-gradient weights from the current parameters
             self.outside_bytes += torch.cuda.memory_allocated(self.device) - mem0
-            self._pack = None                  # the next refresh_weights() covers them too ...
+        elif plan is not self._bwd:
+            plan.refresh()                     # its data-gradient weights are as old as its last run
+        if plan is not self._bwd:
+            self._bwd = plan
+            self._pack = None                  # the next refresh_weights() covers its weights too ...
             self._graphs = {}                  # ... so captured forward graphs (old packing plan) are dropped
-        self._bwd.run(grads)
-        return self._bwd
+        plan.run(grads)
+        return plan

@@ -57,6 +57,8 @@ class Wgrad:
 
 
 PACK_FWD, PACK_DGRAD, PACK_STEM, PACK_DETECT, PACK_DETECT_DGRAD, PACK_DETECT_BIAS, PACK_DGRAD_S2 = range(7)
+# PACK_DGRAD with (group_real, group_pad) = (c0, n), n > 0: only the input channels [c0, c0 + n) of the source weight (the data
+# gradient of part of a Concat); (0, 0): all of them
 
 
 class PackEntry(ctypes.Structure):
@@ -67,7 +69,8 @@ class PackEntry(ctypes.Structure):
 
 class PackPlan:
     """All layers' fp32 parameters -> packed bf16 operand buffers in one launch (after every optimiser step).
-    entries: (kind, src parameter tensor fp32, dst packed tensor, group_real, group_pad); shapes are read off the tensors."""
+    entries: (kind, src parameter tensor fp32, dst packed tensor, group_real, group_pad); shapes are read off the tensors
+    (PACK_DGRAD: group_real, group_pad = the input-channel window c0, n, or 0, 0 for all)."""
 
     def __init__(self, entries, device):
         arr = (PackEntry * len(entries))()
@@ -119,7 +122,10 @@ class FusedSGDEMA:
 
     groups: (g0, g1, g2) parameter lists as train.py:148-156 builds them; grads: {parameter: fp32 gradient tensor} with FIXED
     storage (e.g. views of the backward plan's flat buffer); ema_model: a deep copy whose state_dict mirrors model's.
-    step(lr=(lr0, lr1, lr2), momentum, ema_decay) applies torch.optim.SGD(nesterov=True) arithmetic and the EMA rule."""
+    step(lr=(lr0, lr1, lr2), momentum, ema_decay) applies torch.optim.SGD(nesterov=True) arithmetic and the EMA rule.
+    A parameter with requires_grad False (train.py --freeze) is what torch.optim.SGD makes of a parameter without .grad: it
+    is not moved and has no momentum buffer; the EMA still follows it.  momentum_buffers: {parameter: buffer} to continue
+    from; a trainable parameter without one starts from zeros, which equals torch's clone(grad) on its first step."""
 
     def __init__(self, model, groups, grads, ema_model=None, weight_decay: float = 0.0, momentum_buffers=None):
         self.device = next(model.parameters()).device
@@ -128,11 +134,17 @@ class FusedSGDEMA:
         self.mom, ent, self._keep = {}, [], []
         for gi, plist in enumerate(groups):
             for p in plist:
+                e = ema_sd.get(name_of[id(p)])
+                if not p.requires_grad:   # frozen: EMA only
+                    if e is not None:
+                        ent.append(SgdEntry(p.data_ptr(), None, None, e.data_ptr(), p.numel(), 0.0, -1))
+                        self._keep += [p, e]
+                    continue
                 g = grads[p]
                 assert p.dtype == torch.float32 and g.dtype == torch.float32 and p.is_contiguous() and g.is_contiguous()
-                m = momentum_buffers[p] if momentum_buffers is not None else torch.zeros_like(p)
+                m = momentum_buffers.get(p) if momentum_buffers is not None else None
+                m = torch.zeros_like(p) if m is None else m
                 self.mom[p] = m
-                e = ema_sd.get(name_of[id(p)])
                 ent.append(SgdEntry(p.data_ptr(), g.data_ptr(), m.data_ptr(), e.data_ptr() if e is not None else None, p.numel(),
                                     float(weight_decay) if gi == 1 else 0.0, gi))
                 self._keep += [p, g, m, e]
@@ -194,13 +206,15 @@ class FusedAdamEMA:
     {parameter: {'step', 'exp_avg', 'exp_avg_sq'}} such as optimizer.state; where it holds every parameter the moments are
     adopted in place (fp32, contiguous, on the parameter's device) and the step count is theirs, which must be one count for
     all.  `self.state` is torch.optim.Adam's per-parameter state: the moments the kernel updates and a 'step' that is a view
-    of one CPU fp32 tensor, `step_count`, advanced by one op per step.  step(lr=(lr0, lr1, lr2), betas, eps, ema_decay)."""
+    of one CPU fp32 tensor, `step_count`, advanced by one op per step.  step(lr=(lr0, lr1, lr2), betas, eps, ema_decay).
+    A parameter with requires_grad False (train.py --freeze) is not moved and has no state, as torch.optim.Adam treats a
+    parameter without .grad; the EMA still follows it.  "All or none" and the one step count apply to the trainable ones."""
 
     def __init__(self, model, groups, grads, ema_model=None, weight_decay: float = 0.0, state=None):
         self.device = next(model.parameters()).device
         ema_sd = dict(ema_model.state_dict()) if ema_model is not None else {}
         name_of = {id(p): n for n, p in model.named_parameters()}
-        params = [p for plist in groups for p in plist]
+        params = [p for plist in groups for p in plist if p.requires_grad]
         adopted = [state.get(p) if state is not None else None for p in params]
         n_have = sum(1 for s in adopted if s)
         if n_have not in (0, len(params)):
@@ -214,6 +228,12 @@ class FusedAdamEMA:
         i = 0
         for gi, plist in enumerate(groups):
             for p in plist:
+                if not p.requires_grad:   # frozen: EMA only
+                    e = ema_sd.get(name_of[id(p)])
+                    if e is not None:
+                        ent.append(AdamEntry(p.data_ptr(), None, None, None, e.data_ptr(), p.numel(), 0.0, -1))
+                        self._keep += [p, e]
+                    continue
                 g = grads[p]
                 assert p.dtype == torch.float32 and g.dtype == torch.float32 and p.is_contiguous() and g.is_contiguous()
                 s = adopted[i]

@@ -41,6 +41,19 @@ def param_groups(model):
     return g0, g1, g2
 
 
+def freeze_layers(model, freeze=(0,)):
+    """train.py:126-131 (--freeze): [n] freezes layers 0..n-1, a longer list exactly the layers it names.  A parameter whose
+    name contains f"model.{x}." for a frozen x gets requires_grad False, every other one True.  Returns the frozen names."""
+    freeze = [f"model.{x}." for x in (freeze if len(freeze) > 1 else range(freeze[0]))]
+    frozen = []
+    for k, v in model.named_parameters():
+        v.requires_grad = True
+        if any(x in k for x in freeze):
+            v.requires_grad = False
+            frozen.append(k)
+    return frozen
+
+
 def multi_scale_shape(imgsz: int, gs: int, H: int, W: int, rng: random.Random):
     """train.py:314-318 (--multi-scale) for a batch of H x W images: one draw from `rng` -> (ns_h, ns_w, label_ratio).
     The reference passes float bounds to randrange, which Python 3.12 refuses; their integral values give the draws Python
@@ -102,7 +115,8 @@ class TrainStep:
     """model: yolov5_obb_b200.yolo.Model on a CUDA device, in train() mode.  step(imgs, targets) -> (loss, loss_items)."""
 
     def __init__(self, model, hyp: Optional[dict] = None, batch_size: int = 16, imgsz: int = 1024, ema: bool = True,
-                 warmup_iters: int = 0, multi_scale: bool = False, seed: Optional[int] = None, adam: bool = False):
+                 warmup_iters: int = 0, multi_scale: bool = False, seed: Optional[int] = None, adam: bool = False,
+                 freeze=(0,)):
         """warmup_iters > 0: the warm-up of train.py:305-316 over that many iterations (the reference uses
         max(round(warmup_epochs * batches_per_epoch), 1000)): every group's lr is interpolated from 0 (biases: from
         hyp['warmup_bias_lr']) to lr0 and the momentum from hyp['warmup_momentum'] to hyp['momentum'].
@@ -120,7 +134,15 @@ class TrainStep:
         decay) and g2 added as for SGD; Adam groups have no 'momentum', so the warm-up moves only the learning rates.  The
         fused step (below) keeps torch's own per-parameter state in optimizer.state, so optimizer.state_dict() is the
         reference's checkpoint format, and after optimizer.load_state_dict() the next step continues from the loaded
-        moments and step count."""
+        moments and step count.
+
+        freeze: train.py --freeze, applied by freeze_layers before the optimizer and the EMA are built ([10]: the backbone,
+        [0, 1, 2]: those layers; [0]: nothing).  Frozen parameters stay in their parameter groups; the optimizer leaves them
+        as they are and keeps no state for them, the EMA follows them, and the backward plan computes no gradient that
+        only they would need.  requires_grad may also be changed between steps (unfreezing after some epochs): the next
+        step builds the plan for the new flags.  With adam=True, once a frozen parameter becomes trainable torch.optim.Adam
+        keeps a step count per parameter, which the fused kernel cannot follow: the step then uses torch.optim.Adam and
+        the foreach EMA for the rest of the run."""
         self.model = model
         self.hyp = dict(HYP_FINETUNE_DOTA if hyp is None else hyp)
         nbs = 64
@@ -149,6 +171,9 @@ class TrainStep:
             broadcast_model_state(model, 0)
             if hasattr(model, "_bump_generation"):
                 model._bump_generation()
+        freeze_layers(model, freeze)
+        if not any(p.requires_grad for p in model.parameters()):
+            raise RuntimeError(f"freeze={list(freeze)} freezes every parameter of the model: nothing is left to train")
         g0, g1, g2 = param_groups(model)
         self.adam = bool(adam)
         if self.adam:
@@ -171,6 +196,7 @@ class TrainStep:
         import os
         self._fused = None
         self._fused_state = None
+        self._fused_flags = None
         self._use_fused = (self.accumulate == 1 and os.environ.get("Y5OBB_FUSED_SGD", "1") != "0"
                            and next(model.parameters()).is_cuda and hasattr(model, "_bump_generation"))
         if self.multi_scale:
@@ -202,6 +228,8 @@ class TrainStep:
         loss, items = self.compute_loss(pred, targets)
         loss.backward()                                     # (x WORLD_SIZE of train.py:328 is folded into the SUM below)
         if self.ni - self._last_opt >= self.accumulate:
+            if self._use_fused and self.adam and self._unfrozen():
+                self._leave_fused_adam()
             if self._use_fused:
                 self._fused_step()
             else:
@@ -307,6 +335,18 @@ class TrainStep:
         if pending is not None:
             yield finish(pending)
 
+    def _unfrozen(self) -> bool:
+        """Whether the last backward trained a parameter that the fused table holds as frozen."""
+        flags = self.model._last_train_engine._bwd.trainable
+        return self._fused is not None and any(t and not f for t, f in zip(flags, self._fused_flags))
+
+    def _leave_fused_adam(self):
+        """torch.optim.Adam + the foreach EMA from this step on: each parameter's state gets its own step count."""
+        for st in self.optimizer.state.values():
+            if "step" in st:
+                st["step"] = st["step"].clone()
+        self._use_fused, self._fused = False, None
+
     def _fused_step(self):
         """train.py:336-342 (optimizer.step, zero_grad, ema.update) as one launch over a device-resident tensor table.
         Gradients are read in place from the backward plan's flat fp32 buffer (all-reduced in place first when N > 1);
@@ -323,21 +363,25 @@ class TrainStep:
         key = plan.flat if plan.arena is not None else plan   # (an arena's flat buffer is shared by every shape)
         ema = self.ema.ema if self.ema is not None else None
         opt = self.optimizer
+        # (re)built for the plan's buffer and for its trainable flags: frozen parameters are EMA-only entries
+        rebuild = self._fused is None or self._fused_plan is not key or self._fused_flags != plan.trainable
         if self.adam:
-            if self._fused is None or self._fused_plan is not key or self._fused_state is not opt.state:
+            if rebuild or self._fused_state is not opt.state:
                 groups = [g["params"] for g in opt.param_groups]
                 self._fused = FusedAdamEMA(model, groups, plan.pgrad, ema, weight_decay=self.hyp["weight_decay"],
                                            state=opt.state)
-                self._fused_plan = key
+                self._fused_plan, self._fused_flags = key, plan.trainable
                 for p, s in self._fused.state.items():
                     opt.state[p] = s
                 self._fused_state = opt.state
-        elif self._fused is None or self._fused_plan is not key:
+        elif rebuild:
             groups = [g["params"] for g in opt.param_groups]
             self._fused = FusedSGDEMA(model, groups, plan.pgrad, ema,
                                       weight_decay=self.hyp["weight_decay"], momentum_buffers=getattr(self, "_mom", None))
-            self._mom = self._fused.mom
-            self._fused_plan = key
+            # (the buffers of parameters frozen since are kept: torch's SGD resumes from them after an unfreeze)
+            self._mom = dict(getattr(self, "_mom", None) or {})
+            self._mom.update(self._fused.mom)
+            self._fused_plan, self._fused_flags = key, plan.trainable
             for p, m in self._fused.mom.items():
                 opt.state[p]["momentum_buffer"] = m
         g = opt.param_groups

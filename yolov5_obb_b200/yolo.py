@@ -195,14 +195,15 @@ class _TrainFn(torch.autograd.Function):
     inputs of the node so that autograd accumulates their gradients into `.grad` itself."""
 
     @staticmethod
-    def forward(ctx, eng, x, *params):
+    def forward(ctx, eng, x, trainable, *params):
+        """trainable: requires_grad of every model parameter; params: the parameters that require it."""
         outs = eng.forward(x, getattr(eng, "_refresh_next", False))
-        ctx.eng, ctx.params = eng, params
+        ctx.eng, ctx.trainable, ctx.params = eng, trainable, params
         return tuple(o.detach() for o in outs)
 
     @staticmethod
     def backward(ctx, *grads):
-        plan = ctx.eng.backward(list(grads))
+        plan = ctx.eng.backward(list(grads), ctx.trainable)   # (the plan computes only what the trainable ones need)
         # one clone of the flat buffer: autograd may keep the returned views as .grad (zero_grad(set_to_none=True) makes
         # that copy-free), and the plan rewrites its own buffer every step
         flat = plan.flat.clone()
@@ -210,7 +211,7 @@ class _TrainFn(torch.autograd.Function):
         arena = getattr(ctx.eng, "arena", None)
         (arena if arena is not None else ctx.eng).last_grad_flat = flat
         views = {p: flat[o:o + p.numel()].view(p.shape) for p, o in zip(plan.params, plan.offsets)}
-        return (None, None) + tuple(views.get(p) for p in ctx.params)
+        return (None, None, None) + tuple(views.get(p) for p in ctx.params)
 
 
 class Model(nn.Module):
@@ -345,15 +346,18 @@ class Model(nn.Module):
         self._bump_generation()  # running statistics move (the captured graph bumps no version counter)
         if not torch.is_grad_enabled():
             return eng.forward(x, refresh)
-        params = [p for p in self.parameters() if p.requires_grad]
-        return list(_TrainFn.apply(eng, x, *params))
+        allp = list(self.parameters())
+        trainable = tuple(p.requires_grad for p in allp)
+        params = [p for p, t in zip(allp, trainable) if t]
+        return list(_TrainFn.apply(eng, x, trainable, *params))
 
     def reserve_train_arena(self, B, H_max, W_max, device):
         """Carve the activation, raw-output, Detect-logit and gradient buffers of every training plan on `device` from ONE
         allocation sized for a [B, 3, H_max, W_max] plan (train_engine.TrainArena), and give all of them one flat gradient
         buffer.  Any plan of batch <= B and size <= H_max x W_max then fits: a multi-scale run costs the largest shape's
         buffers once, plus per shape only what the plan reports as `outside_bytes` (BatchNorm vectors, packed weights,
-        graphs).  Running out of memory happens here, at start-up.  Training plans built before the call keep their own
+        graphs).  The arena is sized for the full backward plan, whatever is frozen now, so unfreezing later fits.  Running
+        out of memory happens here, at start-up.  Training plans built before the call keep their own
         buffers; plans bound to an earlier arena are dropped.  Returns the arena."""
         from .train_backward import BackwardPlan
         from .train_engine import TrainArena, TrainEngine, _Carver, flat_layout
