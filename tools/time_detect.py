@@ -100,21 +100,22 @@ def time_ops(reps):
     print(f"sum: generic {tot['generic']:.1f} us, records {tot['records']:.1f} us, bound {tot_bound:.1f} us")
 
 
-def build_probe():
+def build_probe(define="Y5OBB_DETECT_PROBE", out_dir=PROBE_DIR, name="liby5obb_probe.so"):
+    """liby5obb.so's sources compiled with -D`define` into out_dir/name (apart from liby5obb.so)."""
     from yolov5_obb_b200.build import CSRC, NVCC_FLAGS
-    obj = PROBE_DIR / "obj"
+    obj = out_dir / "obj"
     obj.mkdir(parents=True, exist_ok=True)
     srcs = sorted(CSRC.glob("*.cu"))
 
     def cc(s):
-        r = subprocess.run(["nvcc", *NVCC_FLAGS, "-DY5OBB_DETECT_PROBE", "-c", str(s), "-o", str(obj / (s.stem + ".o"))],
+        r = subprocess.run(["nvcc", *NVCC_FLAGS, f"-D{define}", "-c", str(s), "-o", str(obj / (s.stem + ".o"))],
                            capture_output=True, text=True)
         if r.returncode:
             raise RuntimeError(f"nvcc failed for {s.name}:\n{r.stdout}\n{r.stderr}")
 
     with ThreadPoolExecutor(max_workers=os.cpu_count() or 4) as ex:
         list(ex.map(cc, srcs))
-    so = PROBE_DIR / "liby5obb_probe.so"
+    so = out_dir / name
     r = subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", str(so),
                         *[str(obj / (s.stem + ".o")) for s in srcs]], capture_output=True, text=True)
     if r.returncode:

@@ -172,15 +172,72 @@ __device__ __forceinline__ void probe(const ConvK& p, int ti, int ph) {
 __device__ __forceinline__ void probe(const ConvK&, int, int) {}
 #endif
 
+// Y5OBB_CONV_PROBE (tools/time_conv_epilogue.py builds it into a library of its own): thread 0 of every CTA of a MODE_CONV
+// launch adds the clock64 cycles since its previous stamp to the phase that each stamp ends, for its first CPROBE_TILES
+// tiles.  The epilogue loops over 64-column blocks (and the synchronous one over vectors), so a phase is the SUM of its
+// intervals within a tile.  CP_NEXT is the gap from the previous tile's last stamp to this tile's start.
+enum ConvProbePhase : int { CP_NEXT = 0, CP_FULL, CP_MMA, CP_STAGED, CP_RES, CP_STORED, CONV_PROBE_PHASES };
+#ifdef Y5OBB_CONV_PROBE
+constexpr int CPROBE_CTAS = 264, CPROBE_TILES = 64;
+__device__ long long g_cprobe[CPROBE_CTAS][CPROBE_TILES][CONV_PROBE_PHASES];
+__device__ long long g_cprobe_last[CPROBE_CTAS];
+__device__ unsigned g_cprobe_sink;
+__device__ __forceinline__ void cprobe(const ConvK& p, int ti, int ph) {
+  if (p.mode == MODE_CONV && threadIdx.x == 0 && blockIdx.x < CPROBE_CTAS && ti < CPROBE_TILES) {
+    const long long now = clock64();
+    if (ti > 0 || ph != CP_NEXT) g_cprobe[blockIdx.x][ti][ph] += now - g_cprobe_last[blockIdx.x];
+    g_cprobe_last[blockIdx.x] = now;
+  }
+}
+// the same once `v` (a loaded value) has arrived: storing it makes the thread wait for the load
+__device__ __forceinline__ void cprobe_after(const ConvK& p, int ti, int ph, unsigned v) {
+  if (threadIdx.x == 0) g_cprobe_sink = v;
+  cprobe(p, ti, ph);
+}
+#else
+__device__ __forceinline__ void cprobe(const ConvK&, int, int) {}
+__device__ __forceinline__ void cprobe_after(const ConvK&, int, int, unsigned) {}
+#endif
+
 // ---- epilogue of one tile for one consumer warp ----------------------------------------------------------------------
+// A 64-column block of a warp's 16 rows leaves as 16 * VECS 8-column vectors; lane `lane` stores vectors lane + 32 k.
+template <int NI>
+struct StoreVecs {
+  static constexpr int VECS = stg_cols(NI) / 8;     // 8-column vectors per staged row
+  static constexpr int PER_LANE = 16 * VECS / 32;   // vectors per lane and block
+  // blocks whose residual vectors are loaded into registers when the tile starts, so that the loads' latency passes under
+  // the tile's MMAs: the first two for NI = 128, the first one otherwise (none for NI = 96, whose 48 accumulators leave no
+  // room in the two-CTA budget; a second block spills at NI = 256); later blocks load in the epilogue.  DIM: the array
+  // extent (at least 1).
+  static constexpr int PREFETCH = NI == 96 ? 0 : (NI == 128 ? 2 : 1);
+  static constexpr int DIM = PREFETCH > 0 ? PREFETCH : 1;
+};
+
+// residual vector k of this lane in the 64-column block at column cb: what the store loop adds to output vector
+// lane + 32 k; zero where that loop stores nothing (columns past the tile or Cout, pixels past the image)
+template <int NI>
+__device__ __forceinline__ uint4 load_res_vec(const ConvK& p, const TileCoord& c, int row0, int lane, int cb, int k) {
+  constexpr int VECS = StoreVecs<NI>::VECS;
+  const int v = lane + 32 * k;
+  const int row = v / VECS, col = cb + (v % VECS) * 8;
+  const int tr = row0 + row;
+  const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+  const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
+  if (col >= min(p.BN, p.Cout - c.n0) || h >= p.Hout || w >= p.Wout) return make_uint4(0u, 0u, 0u, 0u);
+  return *reinterpret_cast<const uint4*>(p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride +
+                                         (long long)w * p.res_pix_stride + c.n0 + col);
+}
+
 // The warp owns 16 pixel rows (row0 .. row0 + 15 of the tile).  wgmma's accumulator layout gives thread `lane` the rows
 // row0 + lane / 4 (+ 8) and the column pairs 8 j + 2 (lane % 4) (+ 1).  Each 64-column block is activated in registers,
-// staged through shared memory as [16 rows][64] fp32 and leaves in 16-byte vectors per pixel.
-template <int NI>
+// staged through shared memory as [16 rows][64] fp32 and leaves in 16-byte vectors per pixel.  RES (launches with a
+// residual): rpf holds the residual vectors of the first StoreVecs<NI>::PREFETCH blocks, loaded when the tile started.
+template <int NI, bool RES>
 __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg, const float* bias_s,
-                                         int row0, int lane, int ti) {
+                                         const uint4 (&rpf)[StoreVecs<NI>::DIM][StoreVecs<NI>::PER_LANE], int row0,
+                                         int lane, int ti) {
   const int q = lane & 3, r = lane >> 2;
-  constexpr int PITCH = stg_pitch(NI), VECS = stg_cols(NI) / 8;  // 8-column vectors per staged row
+  constexpr int PITCH = stg_pitch(NI), VECS = StoreVecs<NI>::VECS;
   float* theta_s = stg + 16 * PITCH;
   const bool det = p.mode == MODE_DETECT;
   const int nvalid = min(p.BN, (det ? p.det_no : p.Cout - c.n0));
@@ -250,43 +307,89 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
     }
     __syncwarp();
     probe(p, ti, PH_STAGED);
+    cprobe(p, ti, CP_STAGED);
     // (2) 16 rows x (up to) 64 columns leave in vectors
     if (!det) {
-      for (int v = lane; v < 16 * VECS; v += 32) {
-        const int row = v / VECS, col = cb + (v % VECS) * 8;
-        const int tr = row0 + row;
-        const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
-        const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
-        if (col >= nvalid || h >= p.Hout || w >= p.Wout) continue;
-        const float* sp = stg + row * PITCH + (col - cb);
-        const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
-        float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-        const int ch = c.n0 + col;
-        if (p.res) {
-          const uint4 rv = *reinterpret_cast<const uint4*>(p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride +
-                                                            (long long)w * p.res_pix_stride + ch);
-          const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv);
+      if constexpr (RES) {  // vector v = lane + 32 k; k indexes rpf, so the loop is unrolled
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float2 g = __bfloat1622float2(rh[k]);
-            f[2 * k] += g.x;
-            f[2 * k + 1] += g.y;
+        for (int k = 0; k < StoreVecs<NI>::PER_LANE; ++k) {
+          const int v = lane + 32 * k;
+          const int row = v / VECS, col = cb + (v % VECS) * 8;
+          const int tr = row0 + row;
+          const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+          const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
+          if (col >= nvalid || h >= p.Hout || w >= p.Wout) continue;
+          const float* sp = stg + row * PITCH + (col - cb);
+          const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
+          float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+          const int ch = c.n0 + col;
+          if (p.res) {
+            const uint4 rv = cb / 64 < StoreVecs<NI>::PREFETCH ? rpf[cb / 64][k] : load_res_vec<NI>(p, c, row0, lane, cb, k);
+            const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv);
+            cprobe_after(p, ti, CP_RES, rv.x ^ rv.w);
+  #pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float2 g = __bfloat1622float2(rh[k]);
+              f[2 * k] += g.x;
+              f[2 * k + 1] += g.y;
+            }
           }
+          uint4 o;
+          o.x = pack_bf16(f[0], f[1]);
+          o.y = pack_bf16(f[2], f[3]);
+          o.z = pack_bf16(f[4], f[5]);
+          o.w = pack_bf16(f[6], f[7]);
+          *reinterpret_cast<uint4*>(p.out + (long long)c.b * p.out_img_stride + (long long)h * p.out_row_stride +
+                                    (long long)w * p.out_pix_stride + ch) = o;
+          if (p.out2x) {  // nn.Upsample(2x nearest): the same vector on the four (dy, dx) phases
+            const long long px = p.out2x_pix_stride, rw = 2LL * p.Wout * px;
+            __nv_bfloat16* u = p.out2x + (((long long)c.b * 2 * p.Hout + 2 * h) * (2 * p.Wout) + 2 * w) * px + ch;
+            *reinterpret_cast<uint4*>(u) = o;
+            *reinterpret_cast<uint4*>(u + px) = o;
+            *reinterpret_cast<uint4*>(u + rw) = o;
+            *reinterpret_cast<uint4*>(u + rw + px) = o;
+          }
+          cprobe(p, ti, CP_STORED);
         }
-        uint4 o;
-        o.x = pack_bf16(f[0], f[1]);
-        o.y = pack_bf16(f[2], f[3]);
-        o.z = pack_bf16(f[4], f[5]);
-        o.w = pack_bf16(f[6], f[7]);
-        *reinterpret_cast<uint4*>(p.out + (long long)c.b * p.out_img_stride + (long long)h * p.out_row_stride +
-                                  (long long)w * p.out_pix_stride + ch) = o;
-        if (p.out2x) {  // nn.Upsample(2x nearest): the same vector on the four (dy, dx) phases
-          const long long px = p.out2x_pix_stride, rw = 2LL * p.Wout * px;
-          __nv_bfloat16* u = p.out2x + (((long long)c.b * 2 * p.Hout + 2 * h) * (2 * p.Wout) + 2 * w) * px + ch;
-          *reinterpret_cast<uint4*>(u) = o;
-          *reinterpret_cast<uint4*>(u + px) = o;
-          *reinterpret_cast<uint4*>(u + rw) = o;
-          *reinterpret_cast<uint4*>(u + rw + px) = o;
+      } else {
+        for (int v = lane; v < 16 * VECS; v += 32) {
+          const int row = v / VECS, col = cb + (v % VECS) * 8;
+          const int tr = row0 + row;
+          const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+          const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
+          if (col >= nvalid || h >= p.Hout || w >= p.Wout) continue;
+          const float* sp = stg + row * PITCH + (col - cb);
+          const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
+          float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+          const int ch = c.n0 + col;
+          if (p.res) {
+            const uint4 rv = *reinterpret_cast<const uint4*>(p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride +
+                                                              (long long)w * p.res_pix_stride + ch);
+            const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv);
+            cprobe_after(p, ti, CP_RES, rv.x ^ rv.w);
+  #pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float2 g = __bfloat1622float2(rh[k]);
+              f[2 * k] += g.x;
+              f[2 * k + 1] += g.y;
+            }
+          }
+          uint4 o;
+          o.x = pack_bf16(f[0], f[1]);
+          o.y = pack_bf16(f[2], f[3]);
+          o.z = pack_bf16(f[4], f[5]);
+          o.w = pack_bf16(f[6], f[7]);
+          *reinterpret_cast<uint4*>(p.out + (long long)c.b * p.out_img_stride + (long long)h * p.out_row_stride +
+                                    (long long)w * p.out_pix_stride + ch) = o;
+          if (p.out2x) {  // nn.Upsample(2x nearest): the same vector on the four (dy, dx) phases
+            const long long px = p.out2x_pix_stride, rw = 2LL * p.Wout * px;
+            __nv_bfloat16* u = p.out2x + (((long long)c.b * 2 * p.Hout + 2 * h) * (2 * p.Wout) + 2 * w) * px + ch;
+            *reinterpret_cast<uint4*>(u) = o;
+            *reinterpret_cast<uint4*>(u + px) = o;
+            *reinterpret_cast<uint4*>(u + rw) = o;
+            *reinterpret_cast<uint4*>(u + rw + px) = o;
+          }
+          cprobe(p, ti, CP_STORED);
         }
       }
     } else {
@@ -457,8 +560,9 @@ __device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord
   probe(p, ti, PH_STORED);
 }
 
-// RECORDS: the Detect head with compact records (epilogue_records); otherwise epilogue<NI>, which serves every other launch
-template <int NI, bool RECORDS>
+// RECORDS: the Detect head with compact records (epilogue_records); otherwise epilogue<NI, RES>, which serves every other
+// launch.  RES: a MODE_CONV launch with a residual, whose residual vectors are loaded when each tile starts.
+template <int NI, bool RECORDS, bool RES = false>
 __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_kernel(const __grid_constant__ ConvK p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
@@ -590,10 +694,22 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
     uint32_t scale_d = 0u, bres_lo = res_lo;
     int kc = 0;
     probe(p, ti, PH_TILE);
+    cprobe(p, ti, CP_NEXT);
+    uint4 rpf[StoreVecs<NI>::DIM][StoreVecs<NI>::PER_LANE];  // RES: residual vectors, in flight under the MMAs
+    if constexpr (RES) {
+#pragma unroll
+      for (int b = 0; b < StoreVecs<NI>::PREFETCH; ++b)
+#pragma unroll
+        for (int k = 0; k < StoreVecs<NI>::PER_LANE; ++k)
+          rpf[b][k] = load_res_vec<NI>(p, c, wg * 64 + (warp & 3) * 16, lane, 64 * b, k);
+    }
     for (int u0 = 0; u0 < n_units; u0 += group) {
       const int ng = min(group, n_units - u0);
       ptx::mbar_wait(&full_bar[s], ph);
-      if (u0 == 0) probe(p, ti, PH_FULL);
+      if (u0 == 0) {
+        probe(p, ti, PH_FULL);
+        cprobe(p, ti, CP_FULL);
+      }
       ptx::wgmma_fence_regs(acc);
       ptx::wgmma_fence();
       uint32_t u_lo = s_lo;
@@ -635,6 +751,7 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
     if (lane == 0) ptx::mbar_arrive(&empty_bar[prev_s]);
     prev_s = -1;
     probe(p, ti, PH_MMA);
+    cprobe(p, ti, CP_MMA);
     if constexpr (RECORDS) {
       if (c.nt != bt_nt) {  // every consumer warp walks the same tiles, so all of them come here together
         asm volatile("bar.sync 1, %0;" ::"n"(32 * CONSUMER_WARPS) : "memory");  // no warp reads the old anchor's any more
@@ -646,7 +763,7 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
       }
       epilogue_records<NI>(p, c, acc, bt_s, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
     } else {
-      epilogue<NI>(p, c, acc, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
+      epilogue<NI, RES>(p, c, acc, stg, bias_s, rpf, wg * 64 + (warp & 3) * 16, lane, ti);
     }
   }
   if constexpr (RECORDS) ptx::tma_store_wait_all();  // the records' bulk stores complete before the CTA exits
@@ -681,17 +798,18 @@ int instr_n(int bn) { return bn <= 16 ? 16 : (bn + 31) / 32 * 32; }
 
 typedef void (*KernelFn)(ConvK);
 int ctas_for(int ni) { return ni <= 96 ? 2 : 1; }  // Occupancy<NI>::CTAS
+template <bool RES>
 KernelFn kernel_for(int ni) {
   switch (ni) {
-    case 16: return conv_wgmma_kernel<16, false>;
-    case 32: return conv_wgmma_kernel<32, false>;
-    case 64: return conv_wgmma_kernel<64, false>;
-    case 96: return conv_wgmma_kernel<96, false>;
-    case 128: return conv_wgmma_kernel<128, false>;
-    case 160: return conv_wgmma_kernel<160, false>;
-    case 192: return conv_wgmma_kernel<192, false>;
-    case 224: return conv_wgmma_kernel<224, false>;
-    case 256: return conv_wgmma_kernel<256, false>;
+    case 16: return conv_wgmma_kernel<16, false, RES>;
+    case 32: return conv_wgmma_kernel<32, false, RES>;
+    case 64: return conv_wgmma_kernel<64, false, RES>;
+    case 96: return conv_wgmma_kernel<96, false, RES>;
+    case 128: return conv_wgmma_kernel<128, false, RES>;
+    case 160: return conv_wgmma_kernel<160, false, RES>;
+    case 192: return conv_wgmma_kernel<192, false, RES>;
+    case 224: return conv_wgmma_kernel<224, false, RES>;
+    case 256: return conv_wgmma_kernel<256, false, RES>;
     default: return nullptr;
   }
 }
@@ -790,7 +908,9 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
   // compact records take epilogue_records when a record fits the 64-column staging row (nc <= 58)
   const bool records = d->mode == MODE_DETECT && d->det_decode == 2 && d->det_no > 180 &&
                        ((d->det_no - 180 + 1) + 3) / 4 * 4 <= 64 && !(d->flags & Y5OBB_CONV_DETECT_GENERIC);
-  o->fn = records ? records_kernel_for(ni) : kernel_for(ni);
+  const bool res_epi = d->mode == MODE_CONV && d->res;  // residual vectors loaded when each tile starts
+  o->fn = records ? records_kernel_for(ni) : (res_epi ? kernel_for<true>(ni) : kernel_for<false>(ni));
+  const int inst = records ? 1 : (res_epi ? 2 : 0);
   if (!o->fn) {
     delete o;
     return Y5OBB_EINVAL;
@@ -890,8 +1010,8 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     delete o;
     return Y5OBB_EINVAL;
   }
-  static bool attr_set[2][257] = {};  // per instantiation (NI, records)
-  if (!attr_set[records][ni]) {
+  static bool attr_set[3][257] = {};  // per instantiation (NI; plain, records, residual)
+  if (!attr_set[inst][ni]) {
     // all of the unified L1 / shared memory as shared memory, so that two 112 KB CTAs fit beside each other
     cudaError_t e = cudaFuncSetAttribute(o->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
     if (e == cudaSuccess)
@@ -900,7 +1020,7 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
       delete o;
       return cuda_fail(e);
     }
-    attr_set[records][ni] = true;
+    attr_set[inst][ni] = true;
   }
   auto smem_of_plan = [&]() { return k.b_res_bytes + (size_t)k.stages * stage_bytes + fixed_bytes; };
   o->smem = smem_of_plan();
@@ -1083,6 +1203,22 @@ extern "C" int y5obb_detect_probe(void* host, size_t bytes, int* dims) {
   dims[0] = PROBE_CTAS;
   dims[1] = PROBE_TILES;
   dims[2] = PROBE_PHASES;
+  return Y5OBB_OK;
+}
+#endif
+
+#ifdef Y5OBB_CONV_PROBE
+// the conv probe build's per-phase cycle sums (see g_cprobe): copies them to `host` ([CPROBE_CTAS][CPROBE_TILES]
+// [CONV_PROBE_PHASES] int64, `bytes` long) and zeroes them; returns the element count of each dimension in dims[3]
+extern "C" int y5obb_conv_probe(void* host, size_t bytes, int* dims) {
+  if (bytes < sizeof(g_cprobe) || !host || !dims) return Y5OBB_EINVAL;
+  cudaError_t e = cudaMemcpyFromSymbol(host, g_cprobe, sizeof(g_cprobe));
+  static long long zeros[CPROBE_CTAS][CPROBE_TILES][CONV_PROBE_PHASES];
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_cprobe, zeros, sizeof(g_cprobe));
+  if (e != cudaSuccess) return cuda_fail(e);
+  dims[0] = CPROBE_CTAS;
+  dims[1] = CPROBE_TILES;
+  dims[2] = CONV_PROBE_PHASES;
   return Y5OBB_OK;
 }
 #endif
