@@ -6,7 +6,7 @@ into build/conv_probe/ (apart from liby5obb.so) and runs each conv launch of the
 of every CTA sums clock64 cycles per phase of each of its first 64 tiles.  The phases are waiting for the first operands,
 the MMAs, bias/SiLU staged, residual available and stores issued, plus the gap to the next tile.  Printed per op: mean cycles
 per tile for each phase (over CTAs and tiles), then the means of each schedule class.  The probe's stamps cost cycles of their
-own (the synchronous epilogue stamps every vector), so compare phases within a build rather than against CUDA-event times.
+own (the epilogue stamps each 64-column block), so compare phases within a build rather than against CUDA-event times.
 The card's name, power limit and maximum SM clock are printed first.
 """
 import argparse

@@ -46,11 +46,13 @@ constexpr int SMEM_TOTAL = 224 * 1024;                   // dynamic shared memor
 // (correct, but slower); y5obb_conv_schedule and tests/test_conv_schedule_gpu.py expose that.
 constexpr int SMEM_PAIR = 112 * 1024;
 
-// Epilogue staging per consumer warp: 16 rows x min(NI, 64) fp32 columns, each row padded by 4 (spreads the banks), then
-// 16 theta indices.
+// Epilogue staging per consumer warp, sized for the Detect head: 16 rows x min(NI, 64) fp32 columns, each row padded by 4
+// (spreads the banks), then 16 theta indices.  A conv epilogue uses the first half of it: a 16 x min(NI, 64) bf16 output
+// block, then a bf16 residual block of the same shape (see stg_chunk).
 __host__ __device__ constexpr int stg_cols(int ni) { return ni < 64 ? ni : 64; }
 __host__ __device__ constexpr int stg_pitch(int ni) { return stg_cols(ni) + 4; }
 __host__ __device__ constexpr int stg_bytes(int ni) { return (16 * stg_pitch(ni) + 16) * 4; }
+static_assert(2 * 16 * stg_cols(16) * 2 <= stg_bytes(16) && 2 * 16 * stg_cols(64) * 2 <= stg_bytes(64), "conv staging fits");
 
 // Instantiations with NI <= 96 run two CTAs per SM: 2 x 384 threads at 80 registers each, of which setmaxnreg gives the
 // producer warpgroup 32 and the consumers 104 (128 * 32 + 256 * 104 = 384 * 80).  Wider ones keep the SM to themselves,
@@ -174,14 +176,13 @@ __device__ __forceinline__ void probe(const ConvK&, int, int) {}
 
 // Y5OBB_CONV_PROBE (tools/time_conv_epilogue.py builds it into a library of its own): thread 0 of every CTA of a MODE_CONV
 // launch adds the clock64 cycles since its previous stamp to the phase that each stamp ends, for its first CPROBE_TILES
-// tiles.  The epilogue loops over 64-column blocks (and the synchronous one over vectors), so a phase is the SUM of its
-// intervals within a tile.  CP_NEXT is the gap from the previous tile's last stamp to this tile's start.
+// tiles.  The epilogue loops over 64-column blocks, so a phase is the SUM of its intervals within a tile.  CP_NEXT is the
+// gap from the previous tile's last stamp to this tile's start.
 enum ConvProbePhase : int { CP_NEXT = 0, CP_FULL, CP_MMA, CP_STAGED, CP_RES, CP_STORED, CONV_PROBE_PHASES };
 #ifdef Y5OBB_CONV_PROBE
 constexpr int CPROBE_CTAS = 264, CPROBE_TILES = 64;
 __device__ long long g_cprobe[CPROBE_CTAS][CPROBE_TILES][CONV_PROBE_PHASES];
 __device__ long long g_cprobe_last[CPROBE_CTAS];
-__device__ unsigned g_cprobe_sink;
 __device__ __forceinline__ void cprobe(const ConvK& p, int ti, int ph) {
   if (p.mode == MODE_CONV && threadIdx.x == 0 && blockIdx.x < CPROBE_CTAS && ti < CPROBE_TILES) {
     const long long now = clock64();
@@ -190,6 +191,7 @@ __device__ __forceinline__ void cprobe(const ConvK& p, int ti, int ph) {
   }
 }
 // the same once `v` (a loaded value) has arrived: storing it makes the thread wait for the load
+__device__ unsigned g_cprobe_sink;
 __device__ __forceinline__ void cprobe_after(const ConvK& p, int ti, int ph, unsigned v) {
   if (threadIdx.x == 0) g_cprobe_sink = v;
   cprobe(p, ti, ph);
@@ -200,50 +202,214 @@ __device__ __forceinline__ void cprobe_after(const ConvK&, int, int, unsigned) {
 #endif
 
 // ---- epilogue of one tile for one consumer warp ----------------------------------------------------------------------
-// A 64-column block of a warp's 16 rows leaves as 16 * VECS 8-column vectors; lane `lane` stores vectors lane + 32 k.
+// A 64-column block of a warp's 16 rows leaves as 16 * VECS 8-column vectors; lane `lane` stores vectors lane + 32 k, which
+// are chunk lane % VECS of rows lane / VECS + k * ROW_STEP.
 template <int NI>
 struct StoreVecs {
   static constexpr int VECS = stg_cols(NI) / 8;     // 8-column vectors per staged row
   static constexpr int PER_LANE = 16 * VECS / 32;   // vectors per lane and block
-  // blocks whose residual vectors are loaded into registers when the tile starts, so that the loads' latency passes under
-  // the tile's MMAs: the first two for NI = 128, the first one otherwise (none for NI = 96, whose 48 accumulators leave no
-  // room in the two-CTA budget; a second block spills at NI = 256); later blocks load in the epilogue.  DIM: the array
-  // extent (at least 1).
+  static constexpr int ROW_STEP = 32 / VECS;        // rows between a lane's vectors
+  static constexpr int FRAG = stg_cols(NI) / 4;     // bf16 pairs per lane and block in the accumulator layout
+  // blocks whose residual is loaded into registers (FRAG per lane) when the tile starts, so that the loads' latency passes
+  // under the tile's MMAs: the first two for NI = 128, the first one otherwise (none for NI = 96, whose 48 accumulators
+  // leave no room in the two-CTA budget; a second block spills at NI = 256); later blocks load in the epilogue.  DIM: the
+  // array extent (at least 1).
   static constexpr int PREFETCH = NI == 96 ? 0 : (NI == 128 ? 2 : 1);
   static constexpr int DIM = PREFETCH > 0 ? PREFETCH : 1;
 };
 
-// residual vector k of this lane in the 64-column block at column cb: what the store loop adds to output vector
-// lane + 32 k; zero where that loop stores nothing (columns past the tile or Cout, pixels past the image)
+// residual vector k of this lane in the 64-column block at column cb, in the store layout (vector lane + 32 k); nullptr
+// where the store loop stores nothing (columns past the tile or Cout, pixels past the image)
 template <int NI>
-__device__ __forceinline__ uint4 load_res_vec(const ConvK& p, const TileCoord& c, int row0, int lane, int cb, int k) {
+__device__ __forceinline__ const __nv_bfloat16* res_vec(const ConvK& p, const TileCoord& c, int row0, int lane, int cb, int k) {
   constexpr int VECS = StoreVecs<NI>::VECS;
   const int v = lane + 32 * k;
   const int row = v / VECS, col = cb + (v % VECS) * 8;
   const int tr = row0 + row;
   const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
   const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
-  if (col >= min(p.BN, p.Cout - c.n0) || h >= p.Hout || w >= p.Wout) return make_uint4(0u, 0u, 0u, 0u);
-  return *reinterpret_cast<const uint4*>(p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride +
-                                         (long long)w * p.res_pix_stride + c.n0 + col);
+  if (col >= min(p.BN, p.Cout - c.n0) || h >= p.Hout || w >= p.Wout) return nullptr;
+  return p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride + (long long)w * p.res_pix_stride + c.n0 +
+         col;
+}
+// the residual of the 64-column block at column cb in the accumulator layout: rf[2 jj + i] holds row row0 + lane / 4 + 8 i,
+// columns cb + 8 jj + 2 (lane % 4) (+ 1) as bf16x2 (4-byte loads; a quad reads 16 contiguous bytes of a pixel); zero where
+// nothing is stored
+template <int NI>
+__device__ __forceinline__ void load_res_frag(const ConvK& p, const TileCoord& c, int row0, int lane, int cb,
+                                              uint32_t (&rf)[StoreVecs<NI>::FRAG]) {
+  const int nvalid = min(p.BN, p.Cout - c.n0), col = cb + 2 * (lane & 3);
+  const __nv_bfloat16* rp[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int tr = row0 + (lane >> 2) + 8 * i;
+    const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+    const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
+    rp[i] = h < p.Hout && w < p.Wout
+                ? p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride + (long long)w * p.res_pix_stride +
+                      c.n0 + col
+                : nullptr;
+  }
+#pragma unroll
+  for (int jj = 0; jj < StoreVecs<NI>::FRAG / 2; ++jj)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      rf[2 * jj + i] = rp[i] && col + 8 * jj < nvalid ? *reinterpret_cast<const uint32_t*>(rp[i] + 8 * jj) : 0u;
 }
 
-// The warp owns 16 pixel rows (row0 .. row0 + 15 of the tile).  wgmma's accumulator layout gives thread `lane` the rows
-// row0 + lane / 4 (+ 8) and the column pairs 8 j + 2 (lane % 4) (+ 1).  Each 64-column block is activated in registers,
-// staged through shared memory as [16 rows][64] fp32 and leaves in 16-byte vectors per pixel.  RES (launches with a
-// residual): rpf holds the residual vectors of the first StoreVecs<NI>::PREFETCH blocks, loaded when the tile started.
+// Byte offset of 16-byte chunk i (row i / VECS, 8-column group i % VECS) of a conv staging block.  The chunks of each
+// 128-byte line are permuted by XOR with the line's index, so that the eight rows of one column group (an stmatrix /
+// ldmatrix matrix) and eight consecutive chunks (a quarter-warp of the store loop) fall in eight different bank quads.
+__device__ __forceinline__ uint32_t stg_chunk(uint32_t i) { return (i ^ ((i >> 3) & 7u)) << 4; }
+
+// MODE_CONV.  The warp owns 16 pixel rows (row0 .. row0 + 15 of the tile).  wgmma's accumulator layout gives thread
+// `lane` the rows row0 + lane / 4 (+ 8) and the column pairs 8 j + 2 (lane % 4) (+ 1): for each pair of 8-column groups,
+// exactly the four 8 x 8 matrices of one stmatrix.x4.  Per 64-column block: bias (+ SiLU) in registers, the residual
+// (RES) added in fp32 in registers, one rounding to bf16, the block staged as [16 rows][64] bf16 by stmatrix, and 16-byte
+// stores per pixel.  RES: rpf holds the residual of the first StoreVecs<NI>::PREFETCH blocks in the accumulator layout,
+// loaded when the tile started; a later block's residual is copied by cp.async into the staging area's second half in the
+// store layout and comes back in the accumulator layout by ldmatrix.  The probe's phases: CP_STAGED the activation and
+// the staging, CP_RES the wait for the residual, CP_STORED the stores.
 template <int NI, bool RES>
 __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg, const float* bias_s,
-                                         const uint4 (&rpf)[StoreVecs<NI>::DIM][StoreVecs<NI>::PER_LANE], int row0,
+                                         const uint32_t (&rpf)[StoreVecs<NI>::DIM][StoreVecs<NI>::FRAG], int row0,
                                          int lane, int ti) {
-  const int q = lane & 3, r = lane >> 2;
-  constexpr int PITCH = stg_pitch(NI), VECS = StoreVecs<NI>::VECS;
-  float* theta_s = stg + 16 * PITCH;
-  const bool det = p.mode == MODE_DETECT;
-  const int nvalid = min(p.BN, (det ? p.det_no : p.Cout - c.n0));
-  const int nfix = p.det_no - 180;  // Detect: 5 + nc leading columns, then the theta bins
+  constexpr int VECS = StoreVecs<NI>::VECS, PER_LANE = StoreVecs<NI>::PER_LANE, ROW_STEP = StoreVecs<NI>::ROW_STEP;
+  const int q = lane & 3;
+  const int nvalid = min(p.BN, p.Cout - c.n0);
   const float* bias = bias_s + c.n0;
-  if (det && p.det_decode == 2) {
+  const uint32_t out_s = ptx::smem_u32(stg), res_s = out_s + 16 * stg_cols(NI) * 2;
+  // stmatrix / ldmatrix: lane gives the address of row lane % 16 of column group 2 jp + lane / 16
+  const uint32_t mat = (uint32_t)((lane & 15) * VECS + (lane >> 4));
+  // The store loop's vectors of this lane: column vcol of rows lane / VECS + k * ROW_STEP, whose pixels are found once per
+  // tile: hw[k] = (hl << 16) | wl, the pixel's row and column within the tile (-1 past the image), from obase / obase2x.
+  const int vcol = (lane % VECS) * 8;
+  int hw[PER_LANE];
+  __nv_bfloat16* obase;
+  __nv_bfloat16* obase2x;
+#pragma unroll
+  for (int cb = 0; cb < NI; cb += 64) {
+    if (cb >= nvalid) break;
+    const bool prefetched = cb / 64 < StoreVecs<NI>::PREFETCH;
+    if constexpr (RES) {  // a later block's residual is copied here, straight into shared memory, and lands while (1) runs
+      if (!prefetched) {
+#pragma unroll
+        for (int k = 0; k < PER_LANE; ++k) {
+          const __nv_bfloat16* src = res_vec<NI>(p, c, row0, lane, cb, k);
+          ptx::cp_async_16(res_s + stg_chunk(lane + 32 * k), src ? src : p.res, src ? 16u : 0u);
+        }
+      }
+    }
+    // (1) bias (+ SiLU) in registers, in place
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = cb / 8 + jj;
+      if (j < NI / 8) {
+        const int col = 8 * j + 2 * q;
+        const float b0 = bias[col], b1 = bias[col + 1];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float& v0 = acc[4 * j + 2 * i];
+          float& v1 = acc[4 * j + 2 * i + 1];
+          if (p.act) {  // SiLU(x) = h + h * tanh(h), h = x / 2 = 0.5 * acc + (0.5 * bias)
+            const float h0 = fmaf(v0, 0.5f, b0), h1 = fmaf(v1, 0.5f, b1);
+            v0 = fmaf(h0, tanh_fast(h0), h0);
+            v1 = fmaf(h1, tanh_fast(h1), h1);
+          } else {
+            v0 += b0;
+            v1 += b1;
+          }
+        }
+      }
+    }
+    cprobe(p, ti, CP_STAGED);
+    if constexpr (RES) {
+      if (prefetched) {
+        cprobe_after(p, ti, CP_RES, rpf[cb / 64][0] ^ rpf[cb / 64][StoreVecs<NI>::FRAG - 1]);
+      } else {
+        ptx::cp_async_wait_all();
+        cprobe(p, ti, CP_RES);
+        __syncwarp();
+      }
+    }
+    // (2) (+ residual in fp32), one rounding to bf16, staged by stmatrix: matrix m of column-group pair jp is group
+    // 2 jp + m / 2, rows 8 (m % 2) .. 8 (m % 2) + 7
+#pragma unroll
+    for (int jp = 0; jp < 4; ++jp) {
+      const int j0 = cb / 8 + 2 * jp;
+      if (j0 < NI / 8 && 2 * jp < VECS) {
+        uint32_t rb[4];
+        if constexpr (RES) {
+          if (prefetched) {  // (the index stays in range in the unrolled blocks where this branch is dead)
+#pragma unroll
+            for (int m = 0; m < 4; ++m) rb[m] = rpf[prefetched ? cb / 64 : 0][4 * jp + m];
+          } else {
+            ptx::ldmatrix_x4(res_s + stg_chunk(mat + 2 * jp), rb);
+          }
+        }
+        uint32_t o[4];
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          float f0 = acc[4 * (j0 + m / 2) + 2 * (m % 2)], f1 = acc[4 * (j0 + m / 2) + 2 * (m % 2) + 1];
+          if constexpr (RES) {
+            const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb[m]));
+            f0 += g.x;
+            f1 += g.y;
+          }
+          o[m] = pack_bf16(f0, f1);
+        }
+        ptx::stmatrix_x4(out_s + stg_chunk(mat + 2 * jp), o);
+      }
+    }
+    __syncwarp();
+    cprobe(p, ti, CP_STAGED);
+    if (cb == 0) {  // once per tile, after the first block's accumulators are staged (fewer registers live)
+#pragma unroll
+      for (int k = 0; k < PER_LANE; ++k) {
+        const int tr = row0 + lane / VECS + k * ROW_STEP;
+        const int hl = (int)fdiv((uint32_t)tr, p.fd_wt), wl = tr - hl * p.Wt;
+        hw[k] = c.h0 + hl < p.Hout && c.w0 + wl < p.Wout ? (hl << 16) | wl : -1;
+      }
+      obase = p.out + (long long)c.b * p.out_img_stride + (long long)c.h0 * p.out_row_stride + (long long)c.w0 * p.out_pix_stride +
+              c.n0 + vcol;
+      obase2x = p.out2x ? p.out2x + (((long long)c.b * 2 * p.Hout + 2 * c.h0) * (2 * p.Wout) + 2 * c.w0) * p.out2x_pix_stride +
+                              c.n0 + vcol
+                        : nullptr;
+    }
+    // (3) 16 rows x (up to) 64 columns leave in vectors
+    if (cb + vcol < nvalid) {
+#pragma unroll
+      for (int k = 0; k < PER_LANE; ++k) {
+        if (hw[k] < 0) continue;
+        const int hl = hw[k] >> 16, wl = hw[k] & 0xFFFF;
+        const uint4 o = ptx::ld_shared_u4(out_s + stg_chunk(lane + 32 * k));
+        *reinterpret_cast<uint4*>(obase + hl * p.out_row_stride + wl * p.out_pix_stride + cb) = o;
+        if (obase2x) {  // nn.Upsample(2x nearest): the same vector on the four (dy, dx) phases
+          const long long px = p.out2x_pix_stride, rw = 2LL * p.Wout * px;
+          __nv_bfloat16* u = obase2x + (2 * hl * rw + 2 * wl * px) + cb;
+          *reinterpret_cast<uint4*>(u) = o;
+          *reinterpret_cast<uint4*>(u + px) = o;
+          *reinterpret_cast<uint4*>(u + rw) = o;
+          *reinterpret_cast<uint4*>(u + rw + px) = o;
+        }
+      }
+    }
+    cprobe(p, ti, CP_STORED);
+    __syncwarp();
+  }
+}
+
+// MODE_DETECT through the shared epilogue (every Detect launch that is not epilogue_records').  Each 64-column block is
+// activated in registers, staged through shared memory as [16 rows][64] fp32 and leaves as fp32 rows.
+template <int NI>
+__device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg,
+                                                const float* bias_s, int row0, int lane, int ti) {
+  const int q = lane & 3, r = lane >> 2;
+  constexpr int PITCH = stg_pitch(NI);
+  float* theta_s = stg + 16 * PITCH;
+  const int nfix = p.det_no - 180;  // 5 + nc leading columns, then the theta bins
+  const float* bias = bias_s + c.n0;
+  if (p.det_decode == 2) {
     // the theta index of each row: the first maximum of the 180 theta LOGITS (the sigmoid is monotone, so this is the index
     // torch.max returns on the activated values whenever those are distinct)
     float best[2] = {-INFINITY, -INFINITY};
@@ -279,7 +445,7 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
     }
     probe(p, ti, PH_ARGMAX);
   }
-  const int ncols = (det && p.det_decode == 2) ? p.det_rec_w : nvalid;  // columns that leave the kernel
+  const int ncols = p.det_decode == 2 ? p.det_rec_w : min(p.BN, p.det_no);  // columns that leave the kernel
 #pragma unroll
   for (int cb = 0; cb < NI; cb += 64) {
     if (cb >= ncols) break;
@@ -307,135 +473,48 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
     }
     __syncwarp();
     probe(p, ti, PH_STAGED);
-    cprobe(p, ti, CP_STAGED);
-    // (2) 16 rows x (up to) 64 columns leave in vectors
-    if (!det) {
-      if constexpr (RES) {  // vector v = lane + 32 k; k indexes rpf, so the loop is unrolled
+    // (2) Detect, N tile nt == anchor nt.  Output row = b * rows_per_image + row_off + (a * H + h) * W + w (models/yolo.py):
+    // the permute is the store's addressing.  det_decode 2 writes compact records (cx, cy, w, h, obj, cls[nc], theta
+    // index, padding) - everything non_max_suppression_obb reads of a row - instead of the det_no columns.
+    const int a = c.nt;
+    const int rw = p.det_decode == 2 ? p.det_rec_w : p.det_no;
+    for (int v = lane; v < 16 * 16; v += 32) {
+      const int row = v >> 4, col = cb + (v & 15) * 4;
+      const int tr = row0 + row;
+      const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
+      const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
+      if (col >= ncols || h >= p.Hout || w >= p.Wout) continue;
+      const float4 x = *reinterpret_cast<const float4*>(stg + row * PITCH + (col - cb));
+      float f[4] = {x.x, x.y, x.z, x.w};
+      if (p.det_decode) {
 #pragma unroll
-        for (int k = 0; k < StoreVecs<NI>::PER_LANE; ++k) {
-          const int v = lane + 32 * k;
-          const int row = v / VECS, col = cb + (v % VECS) * 8;
-          const int tr = row0 + row;
-          const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
-          const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
-          if (col >= nvalid || h >= p.Hout || w >= p.Wout) continue;
-          const float* sp = stg + row * PITCH + (col - cb);
-          const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
-          float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-          const int ch = c.n0 + col;
-          if (p.res) {
-            const uint4 rv = cb / 64 < StoreVecs<NI>::PREFETCH ? rpf[cb / 64][k] : load_res_vec<NI>(p, c, row0, lane, cb, k);
-            const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv);
-            cprobe_after(p, ti, CP_RES, rv.x ^ rv.w);
-  #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const float2 g = __bfloat1622float2(rh[k]);
-              f[2 * k] += g.x;
-              f[2 * k + 1] += g.y;
-            }
-          }
-          uint4 o;
-          o.x = pack_bf16(f[0], f[1]);
-          o.y = pack_bf16(f[2], f[3]);
-          o.z = pack_bf16(f[4], f[5]);
-          o.w = pack_bf16(f[6], f[7]);
-          *reinterpret_cast<uint4*>(p.out + (long long)c.b * p.out_img_stride + (long long)h * p.out_row_stride +
-                                    (long long)w * p.out_pix_stride + ch) = o;
-          if (p.out2x) {  // nn.Upsample(2x nearest): the same vector on the four (dy, dx) phases
-            const long long px = p.out2x_pix_stride, rw = 2LL * p.Wout * px;
-            __nv_bfloat16* u = p.out2x + (((long long)c.b * 2 * p.Hout + 2 * h) * (2 * p.Wout) + 2 * w) * px + ch;
-            *reinterpret_cast<uint4*>(u) = o;
-            *reinterpret_cast<uint4*>(u + px) = o;
-            *reinterpret_cast<uint4*>(u + rw) = o;
-            *reinterpret_cast<uint4*>(u + rw + px) = o;
-          }
-          cprobe(p, ti, CP_STORED);
-        }
-      } else {
-        for (int v = lane; v < 16 * VECS; v += 32) {
-          const int row = v / VECS, col = cb + (v % VECS) * 8;
-          const int tr = row0 + row;
-          const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
-          const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
-          if (col >= nvalid || h >= p.Hout || w >= p.Wout) continue;
-          const float* sp = stg + row * PITCH + (col - cb);
-          const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
-          float f[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-          const int ch = c.n0 + col;
-          if (p.res) {
-            const uint4 rv = *reinterpret_cast<const uint4*>(p.res + (long long)c.b * p.res_img_stride + (long long)h * p.res_row_stride +
-                                                              (long long)w * p.res_pix_stride + ch);
-            const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&rv);
-            cprobe_after(p, ti, CP_RES, rv.x ^ rv.w);
-  #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const float2 g = __bfloat1622float2(rh[k]);
-              f[2 * k] += g.x;
-              f[2 * k + 1] += g.y;
-            }
-          }
-          uint4 o;
-          o.x = pack_bf16(f[0], f[1]);
-          o.y = pack_bf16(f[2], f[3]);
-          o.z = pack_bf16(f[4], f[5]);
-          o.w = pack_bf16(f[6], f[7]);
-          *reinterpret_cast<uint4*>(p.out + (long long)c.b * p.out_img_stride + (long long)h * p.out_row_stride +
-                                    (long long)w * p.out_pix_stride + ch) = o;
-          if (p.out2x) {  // nn.Upsample(2x nearest): the same vector on the four (dy, dx) phases
-            const long long px = p.out2x_pix_stride, rw = 2LL * p.Wout * px;
-            __nv_bfloat16* u = p.out2x + (((long long)c.b * 2 * p.Hout + 2 * h) * (2 * p.Wout) + 2 * w) * px + ch;
-            *reinterpret_cast<uint4*>(u) = o;
-            *reinterpret_cast<uint4*>(u + px) = o;
-            *reinterpret_cast<uint4*>(u + rw) = o;
-            *reinterpret_cast<uint4*>(u + rw + px) = o;
-          }
-          cprobe(p, ti, CP_STORED);
-        }
-      }
-    } else {
-      // Detect, N tile nt == anchor nt.  Output row = b * rows_per_image + row_off + (a * H + h) * W + w (models/yolo.py):
-      // the permute is the store's addressing.  det_decode 2 writes compact records (cx, cy, w, h, obj, cls[nc], theta
-      // index, padding) - everything non_max_suppression_obb reads of a row - instead of the det_no columns.
-      const int a = c.nt;
-      const int rw = p.det_decode == 2 ? p.det_rec_w : p.det_no;
-      for (int v = lane; v < 16 * 16; v += 32) {
-        const int row = v >> 4, col = cb + (v & 15) * 4;
-        const int tr = row0 + row;
-        const int hl = (int)fdiv((uint32_t)tr, p.fd_wt);
-        const int h = c.h0 + hl, w = c.w0 + (tr - hl * p.Wt);
-        if (col >= ncols || h >= p.Hout || w >= p.Wout) continue;
-        const float4 x = *reinterpret_cast<const float4*>(stg + row * PITCH + (col - cb));
-        float f[4] = {x.x, x.y, x.z, x.w};
-        if (p.det_decode) {
+        for (int k = 0; k < 4; ++k) f[k] = sigmoid_fast(f[k]);
+        if (col == 0) {  // xy, wh (models/yolo.py)
+          f[0] = (f[0] * 2.0f - 0.5f + (float)w) * p.det_stride;
+          f[1] = (f[1] * 2.0f - 0.5f + (float)h) * p.det_stride;
+          f[2] = (f[2] * 2.0f) * (f[2] * 2.0f) * p.det_anchor[2 * a];
+          f[3] = (f[3] * 2.0f) * (f[3] * 2.0f) * p.det_anchor[2 * a + 1];
+          if (p.det_descale) {  // _descale_pred (models/yolo.py:183-198): ATen's `/= s` is a multiply by the fp32 1/s,
+                                // the lr de-flip W - x; _rn so that neither contracts into the decode's FMAs
 #pragma unroll
-          for (int k = 0; k < 4; ++k) f[k] = sigmoid_fast(f[k]);
-          if (col == 0) {  // xy, wh (models/yolo.py)
-            f[0] = (f[0] * 2.0f - 0.5f + (float)w) * p.det_stride;
-            f[1] = (f[1] * 2.0f - 0.5f + (float)h) * p.det_stride;
-            f[2] = (f[2] * 2.0f) * (f[2] * 2.0f) * p.det_anchor[2 * a];
-            f[3] = (f[3] * 2.0f) * (f[3] * 2.0f) * p.det_anchor[2 * a + 1];
-            if (p.det_descale) {  // _descale_pred (models/yolo.py:183-198): ATen's `/= s` is a multiply by the fp32 1/s,
-                                  // the lr de-flip W - x; _rn so that neither contracts into the decode's FMAs
-#pragma unroll
-              for (int k = 0; k < 4; ++k) f[k] = __fmul_rn(f[k], p.det_inv_scale);
-              if (p.det_flip_w > 0.0f) f[0] = __fsub_rn(p.det_flip_w, f[0]);
-            }
-          }
-          if (p.det_decode == 2) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              if (col + k >= nfix) f[k] = col + k == nfix ? theta_s[row] : 0.0f;
+            for (int k = 0; k < 4; ++k) f[k] = __fmul_rn(f[k], p.det_inv_scale);
+            if (p.det_flip_w > 0.0f) f[0] = __fsub_rn(p.det_flip_w, f[0]);
           }
         }
-        const long long orow = (long long)c.b * p.det_rows_per_image + p.det_row_off + ((long long)a * p.Hout + h) * p.Wout + w;
-        float* dst = p.det_out + orow * rw + col;
-        if (!(rw & 3)) {
-          *reinterpret_cast<float4*>(dst) = make_float4(f[0], f[1], f[2], f[3]);
-        } else {  // det_no % 4 != 0 (records are always 4-aligned): rows start 4-byte aligned and the last vector ends the row early
+        if (p.det_decode == 2) {
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            if (col + k < ncols) dst[k] = f[k];
+            if (col + k >= nfix) f[k] = col + k == nfix ? theta_s[row] : 0.0f;
         }
+      }
+      const long long orow = (long long)c.b * p.det_rows_per_image + p.det_row_off + ((long long)a * p.Hout + h) * p.Wout + w;
+      float* dst = p.det_out + orow * rw + col;
+      if (!(rw & 3)) {
+        *reinterpret_cast<float4*>(dst) = make_float4(f[0], f[1], f[2], f[3]);
+      } else {  // det_no % 4 != 0 (records are always 4-aligned): rows start 4-byte aligned and the last vector ends the row early
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          if (col + k < ncols) dst[k] = f[k];
       }
     }
     __syncwarp();
@@ -560,8 +639,9 @@ __device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord
   probe(p, ti, PH_STORED);
 }
 
-// RECORDS: the Detect head with compact records (epilogue_records); otherwise epilogue<NI, RES>, which serves every other
-// launch.  RES: a MODE_CONV launch with a residual, whose residual vectors are loaded when each tile starts.
+// RECORDS: the Detect head with compact records (epilogue_records); otherwise epilogue_detect for the other Detect launches
+// and epilogue<NI, RES> for every conv.  RES: a MODE_CONV launch with a residual, whose residual vectors are loaded when
+// each tile starts.
 template <int NI, bool RECORDS, bool RES = false>
 __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_kernel(const __grid_constant__ ConvK p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -695,13 +775,10 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
     int kc = 0;
     probe(p, ti, PH_TILE);
     cprobe(p, ti, CP_NEXT);
-    uint4 rpf[StoreVecs<NI>::DIM][StoreVecs<NI>::PER_LANE];  // RES: residual vectors, in flight under the MMAs
+    uint32_t rpf[StoreVecs<NI>::DIM][StoreVecs<NI>::FRAG];  // RES: residual fragments, in flight under the MMAs
     if constexpr (RES) {
 #pragma unroll
-      for (int b = 0; b < StoreVecs<NI>::PREFETCH; ++b)
-#pragma unroll
-        for (int k = 0; k < StoreVecs<NI>::PER_LANE; ++k)
-          rpf[b][k] = load_res_vec<NI>(p, c, wg * 64 + (warp & 3) * 16, lane, 64 * b, k);
+      for (int b = 0; b < StoreVecs<NI>::PREFETCH; ++b) load_res_frag<NI>(p, c, wg * 64 + (warp & 3) * 16, lane, 64 * b, rpf[b]);
     }
     for (int u0 = 0; u0 < n_units; u0 += group) {
       const int ng = min(group, n_units - u0);
@@ -762,6 +839,8 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
         bt_nt = c.nt;
       }
       epilogue_records<NI>(p, c, acc, bt_s, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
+    } else if (p.mode == MODE_DETECT) {
+      if constexpr (!RES) epilogue_detect<NI>(p, c, acc, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
     } else {
       epilogue<NI, RES>(p, c, acc, stg, bias_s, rpf, wg * 64 + (warp & 3) * 16, lane, ti);
     }

@@ -31,6 +31,32 @@ __device__ __forceinline__ float2 ld_shared_v2(uint32_t addr) {
   asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ uint4 ld_shared_u4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+// 16 bytes global -> shared without passing through registers (L2 only); src_bytes 0 writes 16 zero bytes and reads
+// nothing.  cp_async_wait_all: this thread's copies have landed.
+__device__ __forceinline__ void cp_async_16(uint32_t smem, const void* gmem, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem), "l"(gmem), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Four 8 x 8 matrices of 16-bit elements between shared memory and the mma / wgmma fragment layout: thread t holds
+// elements 2 (t % 4) and 2 (t % 4) + 1 of row t / 4 of matrix m in r[m]; threads 8 m .. 8 m + 7 give the addresses of
+// matrix m's eight 16-byte rows.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
