@@ -222,21 +222,11 @@ PLANS = [
 ]
 
 
-@pytest.mark.parametrize("size,B,H,W,kind", PLANS)
-def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
-    """Every launch against its own descriptor (tests/convref.py).  Bitwise: every act=False conv (train forward, every dgrad
-    form), raw Detect rows, every wgrad (split-K over the whole pixel axis, the stem's window view, Detect's padded
-    channel groups), out2x against the repeated output.  Theta index of records: the first maximum, exactly.  Within a bound
-    of the epilogue's own approximation, on an exact pre-activation:
-      * SiLU convs: tanh.approx's relative error (2^-11 documented, 2^-10 used) times |h| |tanh h|, h = (acc + bias) / 2,
-        plus the fma's fp32 rounding, then one bf16 rounding of the result (2^-8 |y|); a residual is added in fp32 and the
-        sum rounded once (DESIGN §7), so it adds an fp32 rounding and no second bf16 one;
-      * decoded Detect rows and records: the sigmoid 0.5 tanh.approx(0.5 x) + 0.5 errs by at most half of tanh's error (+ one
-        fp32 rounding), propagated through the decode (x 2 stride for xy, x 8 anchor for wh) plus the fp32 roundings of the
-        decode arithmetic."""
-    torch.manual_seed(2)
+def plan_launches(size, B, H, W, kind):
+    """(conv ops, wgrad ops, what keeps them alive) of the yolov5{size} plan of `kind` (forward, records or train) at B x H x
+    W: every launch the plan makes, in plan order; a train plan's forward convs, Detect convs and backward dgrads."""
     m = build_mirror(size, nc=15, seed=0)
-    convs, wgrads = [], []
+    wgrads = []
     if kind == "train":
         m = m.train().to(DEV)
         eng = TrainEngine(m, B, H, W, DEV)
@@ -250,10 +240,25 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
         assert {id(o) for o in plan.keep if isinstance(o, (ConvOp, Wgrad))} == {id(o) for o in bwd + wgrads}
         s2 = [len(p["dgrad_ops"]) for p in plan.conv_parts if "dgrad_ops" in p and p["lay"].mod.conv.stride[0] == 2]
         assert s2 and all(n == 4 for n in s2), s2
-        convs += bwd
-    else:
-        eng = InferenceEngine(m, B, H, W, DEV, compact_detect=kind == "records")
-        convs = list(eng.convs)
+        return convs + bwd, wgrads, (m, eng, plan)
+    eng = InferenceEngine(m, B, H, W, DEV, compact_detect=kind == "records")
+    return list(eng.convs), wgrads, (m, eng)
+
+
+@pytest.mark.parametrize("size,B,H,W,kind", PLANS)
+def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
+    """Every launch against its own descriptor (tests/convref.py).  Bitwise: every act=False conv (train forward, every dgrad
+    form), raw Detect rows, every wgrad (split-K over the whole pixel axis, the stem's window view, Detect's padded
+    channel groups), out2x against the repeated output.  Theta index of records: the first maximum, exactly.  Within a bound
+    of the epilogue's own approximation, on an exact pre-activation:
+      * SiLU convs: tanh.approx's relative error (2^-11 documented, 2^-10 used) times |h| |tanh h|, h = (acc + bias) / 2,
+        plus the fma's fp32 rounding, then one bf16 rounding of the result (2^-8 |y|); a residual is added in fp32 and the
+        sum rounded once (DESIGN §7), so it adds an fp32 rounding and no second bf16 one;
+      * decoded Detect rows and records: the sigmoid 0.5 tanh.approx(0.5 x) + 0.5 errs by at most half of tanh's error (+ one
+        fp32 rounding), propagated through the decode (x 2 stride for xy, x 8 anchor for wh) plus the fp32 roundings of the
+        decode arithmetic."""
+    torch.manual_seed(2)
+    convs, wgrads, _ = plan_launches(size, B, H, W, kind)
     st = _stats()
     for i, op in enumerate(convs):
         check_conv(op, st, f"conv {i}")
@@ -298,14 +303,18 @@ def _check_flat(plan, dwv, want, snap, what):
 
 
 def test_backward_composition_exact():
-    """yolov5m, b8, 1024x1024 (the benchmarked train step) with integer weights: every layer's dgrad launches, run on
-    integer dz, equal conv2d_input of the FORWARD weight with the layer's stride and padding (onto the integers gx held
-    when the plan accumulates there, over a sentinel when it overwrites); each stride-2 phase changes only pixels of its
-    parity; every wgrad equals conv2d_weight (the stem's in the space-to-depth layout, Detect's without the padding
-    channels of its dz).  Bitwise."""
+    """yolov5m, b8, 1024x1024 (the benchmarked train step): backward_composition."""
+    backward_composition("m", 8, 1024, 1024)
+
+
+def backward_composition(size, B, H, W):
+    """The yolov5{size} B x H x W train plan with integer weights: every layer's dgrad launches, run on integer dz, equal
+    conv2d_input of the FORWARD weight with the layer's stride and padding (onto the integers gx held when the plan
+    accumulates there, over a sentinel when it overwrites); each stride-2 phase changes only pixels of its parity; every
+    wgrad equals conv2d_weight (the stem's in the space-to-depth layout, Detect's without the padding channels of its dz).
+    Bitwise.  Returns (dgrad layers, accumulating ones, wgrad layers)."""
     torch.manual_seed(3)
-    B, H, W = 8, 1024, 1024
-    m = build_mirror("m", nc=15, seed=0).train().to(DEV)
+    m = build_mirror(size, nc=15, seed=0).train().to(DEV)
     eng = TrainEngine(m, B, H, W, DEV)
     plan = BackwardPlan(eng)
     with torch.no_grad():
@@ -416,9 +425,10 @@ def test_backward_composition_exact():
         n_wgrad += 1
         shp = x.view().shape
         dgrad(part, lambda: (real @ wf).view(shp[0], shp[1], shp[2], x.C).permute(0, 3, 1, 2), what)
-    print(f"\nyolov5m b8 1024x1024 backward composition: {n_dgrad} dgrad layers ({n_acc} accumulating) and {n_wgrad} wgrad "
-          f"layers bitwise")
+    print(f"\nyolov5{size} b{B} {H}x{W} backward composition: {n_dgrad} dgrad layers ({n_acc} accumulating) and {n_wgrad} "
+          f"wgrad layers bitwise")
     assert n_wgrad == len(plan.conv_parts) + len(plan.det_parts)
+    return n_dgrad, n_acc, n_wgrad
 
 
 def test_backward_stream_schedule(monkeypatch):
