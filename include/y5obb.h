@@ -330,6 +330,12 @@ typedef struct {
 } y5obb_wgrad_desc;
 int y5obb_wgrad_create(const y5obb_wgrad_desc* desc, y5obb_wgrad_t** out);
 int y5obb_wgrad_run(const y5obb_wgrad_t* w, void* stream);
+/* The launch plan y5obb_wgrad_create chose: grid (CTAs), pixels per block bk (64 / 128) as a kwp x khp box, taps per CTA T
+   over ngroups tap groups, input channels per CTA BN in b_chunks 64-column chunks over ci_blks blocks, co_blks 128-row
+   output-channel blocks of a_chunks 64-row chunks, the split-K factor ksplit over `steps` pixel blocks, pipeline stages.
+   Any pointer may be NULL. */
+int y5obb_wgrad_schedule(const y5obb_wgrad_t* w, int* grid, int* bk, int* kwp, int* khp, int* T, int* ngroups, int* BN,
+                         int* b_chunks, int* ci_blks, int* co_blks, int* a_chunks, int* ksplit, int* steps, int* stages);
 void y5obb_wgrad_destroy(y5obb_wgrad_t* w);
 
 /* backward helpers of the training graph (NHWC bf16 gradients):

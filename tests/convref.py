@@ -178,6 +178,13 @@ def conv_reference(op) -> List[Written]:
             val[..., c] = (sig[..., c] * 2) ** 2 * a_
             tol[..., c] = 8 * a_ * es[..., c] * (1 + es[..., c])
         tol = tol * (1 + 1e-6) + 4 * F32_REL * (val.abs() + st)   # the fp32 roundings of the decode arithmetic
+        if d.det_descale:  # test-time augmentation: x y w h times the fp32 1 / s, then x = flip_w - x (two more roundings)
+            inv = d.det_inv_scale   # (the descriptor's fp32 value)
+            val[..., :4] *= inv
+            tol[..., :4] = tol[..., :4] * inv * (1 + F32_REL) + F32_REL * val[..., :4].abs()
+            if d.det_flip_w > 0:
+                val[..., 0] = d.det_flip_w - val[..., 0]
+                tol[..., 0] = tol[..., 0] * (1 + F32_REL) + F32_REL * val[..., 0].abs()
         if d.det_decode == 2:
             theta = p5[..., nfix:].argmax(-1).double()   # the FIRST maximum (torch.argmax's documented rule)
             rec = torch.zeros(val.shape[:-1] + (rec_w,), dtype=torch.float64, device=pre.device)

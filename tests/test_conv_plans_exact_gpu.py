@@ -22,10 +22,11 @@ import torch
 from tests.convref import conv_reference, expected, view_at, wgrad_reference
 from tests.modelgen import build_mirror
 from yolov5_obb_b200.conv import BIAS_HALVED, MODE_DETECT, Conv as ConvOp, Slice, WindowView
-from yolov5_obb_b200.engine import InferenceEngine
+from yolov5_obb_b200.engine import InferenceEngine, TTAPlan
 from yolov5_obb_b200.train_backward import BackwardPlan
-from yolov5_obb_b200.train_engine import TrainEngine
+from yolov5_obb_b200.train_engine import TrainArena, TrainEngine, _Carver
 from yolov5_obb_b200.train_ops import Wgrad
+from yolov5_obb_b200.train_step import freeze_layers
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -222,31 +223,69 @@ PLANS = [
 ]
 
 
-def plan_launches(size, B, H, W, kind):
-    """(conv ops, wgrad ops, what keeps them alive) of the yolov5{size} plan of `kind` (forward, records or train) at B x H x
-    W: every launch the plan makes, in plan order; a train plan's forward convs, Detect convs and backward dgrads."""
+class AliasCarver(_Carver):
+    """A TrainEngine allocator for plans that are only read, never run: the buffers overlap in one shared allocation, so a
+    plan's descriptors and schedules exist without its activations.  Buffer k starts 256 k bytes in (256-byte aligned as
+    the arena carves them, and a start of its own: the plans tell buffers apart by their address); the offsets are counted
+    as the arena counts them, and channel slices keep their offsets within their buffer.  Nothing may run on such a plan."""
+
+    def __init__(self, device):
+        super().__init__(None, device)
+        self.buf = torch.empty(0, dtype=torch.uint8, device=device)
+        self.n = 0
+
+    def take(self, shape, dtype):
+        n = math.prod(int(s) for s in shape) * torch.empty((), dtype=dtype).element_size()
+        a = TrainArena.ALIGN
+        self.off = (self.off + a - 1) // a * a + n
+        start = self.n * a
+        self.n += 1
+        if start + n > self.buf.numel():   # (views of the old allocation keep it alive)
+            self.buf = torch.empty(max(start + n, 2 * self.buf.numel()) + 1024 * a, dtype=torch.uint8, device=self.device)
+        return self.buf[start:start + n].view(dtype).view(tuple(shape))
+
+
+def plan_launches(size, B, H, W, kind, freeze=None, key_only=False):
+    """(conv ops, wgrad ops, what keeps them alive) of the yolov5{size} plan of `kind` at B x H x W, each built by the code
+    path its entry point uses: every launch the plan makes, in plan order.
+      forward / records   InferenceEngine (Model.forward; detect_records, SceneDetector, run_images);
+      tta / tta-records   the three InferenceEngines of TTAPlan (forward_augment; detect_records(augment=True));
+      train               TrainEngine's forward convs and Detect convs, then the dgrads of the BackwardPlan that
+                          TrainEngine.backward builds for the requires_grad flags train.py --freeze `freeze` leaves
+                          (None: every parameter trains).  A multi-scale size is a train plan of that size.
+    key_only: a train plan's buffers all alias one allocation (AliasCarver): its launches can be read but not run."""
     m = build_mirror(size, nc=15, seed=0)
     wgrads = []
     if kind == "train":
         m = m.train().to(DEV)
-        eng = TrainEngine(m, B, H, W, DEV)
-        plan = BackwardPlan(eng)
+        if freeze is not None:
+            freeze_layers(m, [freeze] if isinstance(freeze, int) else list(freeze))
+        eng = TrainEngine(m, B, H, W, DEV, carver=AliasCarver(torch.device(DEV)) if key_only else None)
+        plan = BackwardPlan(eng, tuple(p.requires_grad for p in m.parameters()))
         convs = [lay.conv for lay in eng.conv_layers] + list(eng.det_convs)
         bwd = []
         for part in plan.det_parts + plan.conv_parts:
             bwd += part.get("dgrad_ops", [])
-            wgrads.append(part["wgrad"])
+            if "wgrad" in part:
+                wgrads.append(part["wgrad"])
         # the parts list every conv / wgrad object the backward plan keeps
         assert {id(o) for o in plan.keep if isinstance(o, (ConvOp, Wgrad))} == {id(o) for o in bwd + wgrads}
         s2 = [len(p["dgrad_ops"]) for p in plan.conv_parts if "dgrad_ops" in p and p["lay"].mod.conv.stride[0] == 2]
         assert s2 and all(n == 4 for n in s2), s2
+        if freeze is None:
+            assert len(wgrads) == len(plan.det_parts) + len(plan.conv_parts)
         return convs + bwd, wgrads, (m, eng, plan)
+    assert freeze is None and not key_only
+    if kind in ("tta", "tta-records"):
+        tta = TTAPlan(m, B, H, W, DEV, compact_detect=kind == "tta-records")
+        return [op for e in tta.engines for op in e.convs], wgrads, (m, tta)
+    assert kind in ("forward", "records"), kind
     eng = InferenceEngine(m, B, H, W, DEV, compact_detect=kind == "records")
     return list(eng.convs), wgrads, (m, eng)
 
 
 @pytest.mark.parametrize("size,B,H,W,kind", PLANS)
-def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
+def test_every_launch_matches_its_descriptor(size, B, H, W, kind, freeze=None):
     """Every launch against its own descriptor (tests/convref.py).  Bitwise: every act=False conv (train forward, every dgrad
     form), raw Detect rows, every wgrad (split-K over the whole pixel axis, the stem's window view, Detect's padded
     channel groups), out2x against the repeated output.  Theta index of records: the first maximum, exactly.  Within a bound
@@ -258,7 +297,7 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
         fp32 rounding), propagated through the decode (x 2 stride for xy, x 8 anchor for wh) plus the fp32 roundings of the
         decode arithmetic."""
     torch.manual_seed(2)
-    convs, wgrads, _ = plan_launches(size, B, H, W, kind)
+    convs, wgrads, _ = plan_launches(size, B, H, W, kind, freeze)
     st = _stats()
     for i, op in enumerate(convs):
         check_conv(op, st, f"conv {i}")
@@ -267,9 +306,9 @@ def test_every_launch_matches_its_descriptor(size, B, H, W, kind):
     print(f"\n{size} b{B} {H}x{W} {kind}: {st['conv']} conv and {st['wgrad']} wgrad "
           f"launches checked; {st['bitwise']} bitwise, {st['tolerance']} within the epilogue bound "
           f"(worst {st['worst']:.3f} of it)" + (f"; theta ties in {st['ties']} of {st['rows']} records rows"
-                                                   if kind == "records" else ""))
+                                                   if kind.endswith("records") else ""))
     assert st["conv"] == len(convs) and st["wgrad"] == len(wgrads)
-    if kind == "records":
+    if kind.endswith("records"):
         assert st["ties"] > 0
 
 

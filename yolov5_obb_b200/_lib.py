@@ -65,6 +65,7 @@ PROTOTYPES = {
                                   c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p]),
     "y5obb_wgrad_create": (c_int, [c_void_p, ctypes.POINTER(c_void_p)]),
     "y5obb_wgrad_run": (c_int, [c_void_p, c_void_p]),
+    "y5obb_wgrad_schedule": (c_int, [c_void_p] + [ctypes.POINTER(c_int)] * 14),
     "y5obb_wgrad_destroy": (None, [c_void_p]),
     "y5obb_sgd_ema_plan_create": (c_int, [c_void_p, c_int, ctypes.POINTER(c_void_p)]),
     "y5obb_sgd_ema_plan_run": (c_int, [c_void_p, c_void_p, c_float, c_float, c_int, c_void_p]),

@@ -385,6 +385,28 @@ int y5obb_wgrad_run(const y5obb_wgrad_t* w, void* stream) {
   return Y5OBB_OK;
 }
 
+int y5obb_wgrad_schedule(const y5obb_wgrad_t* w, int* grid, int* bk, int* kwp, int* khp, int* T, int* ngroups, int* BN,
+                         int* b_chunks, int* ci_blks, int* co_blks, int* a_chunks, int* ksplit, int* steps, int* stages) {
+  if (!w) return Y5OBB_EINVAL;
+  const WgradObj* o = reinterpret_cast<const WgradObj*>(w);
+  const WgradK& k = o->k;
+  if (grid) *grid = o->grid;
+  if (bk) *bk = k.bk;
+  if (kwp) *kwp = k.kwp;
+  if (khp) *khp = k.khp;
+  if (T) *T = k.T;
+  if (ngroups) *ngroups = k.ngroups;
+  if (BN) *BN = k.BN;
+  if (b_chunks) *b_chunks = k.b_chunks;
+  if (ci_blks) *ci_blks = k.ci_blks;
+  if (co_blks) *co_blks = k.co_blks;
+  if (a_chunks) *a_chunks = k.a_chunks;
+  if (ksplit) *ksplit = k.ksplit;
+  if (steps) *steps = k.steps;
+  if (stages) *stages = k.stages;
+  return Y5OBB_OK;
+}
+
 void y5obb_wgrad_destroy(y5obb_wgrad_t* w) { delete reinterpret_cast<WgradObj*>(w); }
 
 }  // extern "C"

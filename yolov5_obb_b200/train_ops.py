@@ -46,6 +46,17 @@ class Wgrad:
         rc = _lib.lib().y5obb_wgrad_run(self._h, stream if stream is not None else _lib.stream_ptr(self.device))
         _lib.check(rc, "y5obb_wgrad_run")
 
+    SCHEDULE = ("grid", "bk", "kwp", "khp", "T", "ngroups", "BN", "b_chunks", "ci_blks", "co_blks", "a_chunks", "ksplit",
+                "steps", "stages")
+
+    def info(self) -> dict:
+        """The launch plan the kernel runs (y5obb_wgrad_schedule): grid, pixel block bk = kwp x khp, taps per CTA T and tap
+        groups, input-channel block BN (b_chunks chunks, ci_blks blocks), co_blks output-channel blocks of a_chunks chunks,
+        split-K factor, pixel blocks `steps` and pipeline stages."""
+        v = [c_int() for _ in self.SCHEDULE]
+        _lib.check(_lib.lib().y5obb_wgrad_schedule(self._h, *[ctypes.byref(x) for x in v]), "y5obb_wgrad_schedule")
+        return {n: x.value for n, x in zip(self.SCHEDULE, v)}
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h:
