@@ -45,14 +45,28 @@ def _conv_params(m):
     return fold_bn(m.conv, getattr(m, "bn", None))
 
 
+def stage_input(x: torch.Tensor, x_s2d: torch.Tensor) -> None:
+    """The stem layout pass: x [B, 3, H, W] contiguous fp32 in [0, 1] or uint8 (the caller-side `/ 255` is folded in) ->
+    the space-to-depth stem input x_s2d, on the current stream."""
+    B, _, H, W = x.shape
+    L, st = _lib.lib(), _lib.stream_ptr(x_s2d.device)
+    if x.dtype == torch.uint8:
+        _lib.check(L.y5obb_stem_s2d_u8(x.data_ptr(), x_s2d.data_ptr(), B, H, W, 1, st), "y5obb_stem_s2d_u8")
+    else:
+        _lib.check(L.y5obb_stem_s2d(x.data_ptr(), x_s2d.data_ptr(), B, H, W, 1, st), "y5obb_stem_s2d")
+
+
 class InferenceEngine:
     def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, conv_flags: int = 0, compact_detect: bool = False,
-                 det_out: Optional[torch.Tensor] = None, det_row_base: int = 0, levels=None, descale=None):
-        """The keyword options let several plans write one output (TTAPlan); their defaults give the plain plan:
+                 det_out: Optional[torch.Tensor] = None, det_row_base: int = 0, levels=None, descale=None,
+                 x_s2d: Optional[torch.Tensor] = None):
+        """The keyword options let several plans write one output (TTAPlan, EnsemblePlan); their defaults give the plain plan:
         det_out       an external [B, rows_per_image, no | rec_w] fp32 tensor the Detect epilogue writes into, from row
                       `det_row_base` of every image on (default: an engine-owned tensor holding exactly this plan's rows);
         levels        the Detect levels to emit (default all).  Ops whose outputs reach no kept level are not emitted;
-        descale       (inv_scale, flip_w): the Detect epilogue de-scales x y w h and de-flips x (y5obb_conv_desc.det_descale)."""
+        descale       (inv_scale, flip_w): the Detect epilogue de-scales x y w h and de-flips x (y5obb_conv_desc.det_descale);
+        x_s2d         an external stem input [B, H/2, W/2 + 2, 16] bf16 whose two padding columns are zero (default: an
+                      engine-owned zeroed one).  Plans that share it read one staged image (EnsemblePlan)."""
         device = torch.device(device)
         if device.type != "cuda":
             raise RuntimeError("InferenceEngine needs a CUDA device (sm_90a); there is no CPU path")
@@ -121,7 +135,16 @@ class InferenceEngine:
         # ---- pass 3: emit ops
         # space-to-depth image with one zero pixel of padding left and right of every row: the stem's three
         # horizontal taps are then 48 CONTIGUOUS channels of an overlapping-window view (pixel stride 16)
-        self.x_s2d = torch.zeros((B, H // 2, W // 2 + 2, 16), dtype=torch.bfloat16, device=device)
+        s2d_shape = (B, H // 2, W // 2 + 2, 16)
+        if x_s2d is None:
+            self.x_s2d = torch.zeros(s2d_shape, dtype=torch.bfloat16, device=device)
+        else:
+            _lib.require_cuda(x_s2d, "x_s2d")
+            if (tuple(x_s2d.shape) != s2d_shape or x_s2d.dtype != torch.bfloat16 or not x_s2d.is_contiguous()
+                    or x_s2d.device != device):
+                raise RuntimeError(f"x_s2d must be a contiguous bf16 {list(s2d_shape)} tensor on {device}, got "
+                                   f"{tuple(x_s2d.shape)} {x_s2d.dtype} on {x_s2d.device}")
+            self.x_s2d = x_s2d
         self.keep.append(self.x_s2d)
         self.op_layers = []    # per op: the top-level layer index it belongs to, ("Detect", level) for the head convs
         cur = [None]
@@ -236,17 +259,8 @@ class InferenceEngine:
         _lib.require_cuda(x, "x")
         if tuple(x.shape) != (self.B, 3, self.H, self.W):
             raise RuntimeError(f"engine was planned for {(self.B, 3, self.H, self.W)}, got {tuple(x.shape)}")
-        st = _lib.stream_ptr(self.device)
-        L = _lib.lib()
         with torch.cuda.device(self.device):
-            if x.dtype == torch.uint8:  # raw image: the caller-side `/ 255` is folded into the layout pass
-                x = x.contiguous()
-                _lib.check(L.y5obb_stem_s2d_u8(x.data_ptr(), self.x_s2d.data_ptr(), self.B, self.H, self.W, 1, st),
-                           "y5obb_stem_s2d_u8")
-            else:
-                x = x.contiguous().float()
-                _lib.check(L.y5obb_stem_s2d(x.data_ptr(), self.x_s2d.data_ptr(), self.B, self.H, self.W, 1, st),
-                           "y5obb_stem_s2d")
+            stage_input(x.contiguous() if x.dtype == torch.uint8 else x.contiguous().float(), self.x_s2d)
             return self._run_layers()
 
     def forward_s2d(self) -> torch.Tensor:
@@ -320,9 +334,12 @@ class TTAPlan:
     write them into one shared [B, rows_total, no] (or compact-record) tensor at the branch's row offset, so that the
     torch.cat of the clipped branches is never formed.  Branch 0 runs the plain stem layout pass; branches 1 and 2 resample
     the input into their stem buffer (y5obb_scale_img_s2d) and run forward_s2d().  Every plan skips the ops that feed only the
-    Detect level _clip_augmented drops.  All work is on the current stream; each engine replays its own CUDA graph."""
+    Detect level _clip_augmented drops.  All work is on the current stream; each engine replays its own CUDA graph.
+    As InferenceEngine, the plan can write into an external det_out from row det_row_base on, and `stems` (one entry per
+    branch, None = engine-owned) gives its engines external stem inputs, so that several plans share them (EnsemblePlan)."""
 
-    def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, compact_detect: bool = False, conv_flags: int = 0):
+    def __init__(self, model: "Y.Model", B: int, H: int, W: int, device, compact_detect: bool = False, conv_flags: int = 0,
+                 det_out: Optional[torch.Tensor] = None, det_row_base: int = 0, stems=None):
         device = torch.device(device)
         if device.type != "cuda":
             raise RuntimeError("TTAPlan needs a CUDA device (sm_90a); there is no CPU path")
@@ -334,12 +351,19 @@ class TTAPlan:
         self.nc, self.no = det.nc, det.no
         self.rec_w = ((det.nc + 6) + 3) // 4 * 4
         self.compact_detect = bool(compact_detect)
-        self.pred = torch.empty((B, self.rows_total, self.rec_w if compact_detect else det.no), dtype=torch.float32,
-                                device=device)
+        if det_out is None:
+            if det_row_base:
+                raise RuntimeError("det_row_base needs an external det_out")
+            det_out = torch.empty((B, self.rows_total, self.rec_w if compact_detect else det.no), dtype=torch.float32,
+                                  device=device)
+        self.pred = det_out
+        stems = [None] * len(self.branches) if stems is None else list(stems)
+        if len(stems) != len(self.branches):
+            raise RuntimeError(f"stems needs one entry per branch ({len(self.branches)}), got {len(stems)}")
         self.engines = [InferenceEngine(model, B, g["Hp"], g["Wp"], device, conv_flags, compact_detect, det_out=self.pred,
-                                        det_row_base=g["row_off"], levels=g["levels"],
-                                        descale=None if g["scale"] == 1 else (g["inv_scale"], g["flip_w"]))
-                        for g in self.branches]
+                                        det_row_base=int(det_row_base) + g["row_off"], levels=g["levels"],
+                                        descale=None if g["scale"] == 1 else (g["inv_scale"], g["flip_w"]), x_s2d=xs)
+                        for g, xs in zip(self.branches, stems)]
         self.flops = sum(e.flops for e in self.engines)
 
     def resample_bytes(self, k: int, itemsize: int = 4) -> float:
@@ -366,4 +390,107 @@ class TTAPlan:
             for k in range(1, len(self.engines)):
                 self.resample(x, k)
                 self.engines[k].forward_s2d()
+        return self.pred
+
+
+# ---- model ensembles (models/experimental.py:74-87 Ensemble: the members' rows concatenated along dim 1, one NMS after)
+def ensemble_layout(models, H: int, W: int, augment: bool = False):
+    """Host row layout of an ensemble's output for an H x W input: the members' rows in list order, each member's in its own
+    level order - with augment=True its own _forward_augment branches, padded to its OWN largest stride (yolo.py:152), so a
+    P5 and a P6 member pad their 0.83 / 0.67 branches to multiples of 32 and 64.  H and W must be multiples of the largest
+    stride of all members (DetectMultiBackend sizes images by it).  Returns (per-member first row, rows per image)."""
+    models = list(models)
+    smax = max(int(max(m.stride)) for m in models)
+    if H % smax or W % smax or H <= 0 or W <= 0:
+        raise RuntimeError(f"image size {H}x{W} must be a multiple of the ensemble's largest stride {smax}")
+    bases, row = [], 0
+    for m in models:
+        det = m.model[-1]
+        strides = [int(s) for s in det.stride]
+        if augment:
+            rows = tta_geometry(H, W, int(max(m.stride)), det.nl, det.na, strides)[1]
+        else:
+            rows = sum(det.na * (H // s) * (W // s) for s in strides)
+        bases.append(row)
+        row += rows
+    return bases, row
+
+
+class EnsemblePlan:
+    """Ensemble.forward / forward_augment / detect_records on the device: one plan per member (InferenceEngine, or TTAPlan for
+    augment=True) whose Detect epilogues write the member's rows into one shared [B, rows_total, no] (or compact-record)
+    tensor from the member's row base on, so the torch.cat of the members' outputs is never formed.  The image is staged
+    once (one stem layout pass into `x_s2d`) and every member's stem reads it; with augment=True the scale-1 branches read it
+    too, and each resampled branch input is made once per (scale, member gs) and read by every member with that gs.
+    `steps` lists what forward runs, in order, as (label, fn(x)): ("stem",), ("resample", branch, gs), ("layers", member,
+    branch).  All work is on the current stream; each engine replays its own CUDA graph."""
+
+    def __init__(self, models, B: int, H: int, W: int, device, compact_detect: bool = False, augment: bool = False,
+                 conv_flags: int = 0):
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("EnsemblePlan needs a CUDA device (sm_90a); there is no CPU path")
+        models = list(models)
+        if not models:
+            raise RuntimeError("an ensemble needs at least one member")
+        ncs = sorted({int(m.model[-1].nc) for m in models})
+        if len(ncs) != 1:
+            raise RuntimeError(f"ensemble members have different class counts {ncs}: their rows cannot be concatenated")
+        require_nc(ncs[0], "EnsemblePlan")
+        self.row_bases, self.rows_total = ensemble_layout(models, H, W, augment)
+        self.device, self.B, self.H, self.W = device, B, H, W
+        self.nc = ncs[0]
+        self.no = self.nc + 185
+        self.rec_w = ((self.nc + 6) + 3) // 4 * 4
+        self.compact_detect, self.augment = bool(compact_detect), bool(augment)
+        self.pred = torch.empty((B, self.rows_total, self.rec_w if compact_detect else self.no), dtype=torch.float32,
+                                device=device)
+        self.x_s2d = torch.zeros((B, H // 2, W // 2 + 2, 16), dtype=torch.bfloat16, device=device)
+        self.steps = [(("stem",), lambda x: stage_input(x, self.x_s2d))]
+        if not augment:
+            self.members = [InferenceEngine(m, B, H, W, device, conv_flags, compact_detect, det_out=self.pred,
+                                            det_row_base=base, x_s2d=self.x_s2d)
+                            for m, base in zip(models, self.row_bases)]
+            for i, e in enumerate(self.members):
+                self.steps.append((("layers", i, 0), lambda x, e=e: e.forward_s2d()))
+        else:
+            gss = [int(max(m.stride)) for m in models]
+            stems = {}   # gs -> per branch stem input; branch 0 (scale 1, no padding) is the staged image itself
+            for gs in sorted(set(gss)):
+                stems[gs] = [self.x_s2d] + [torch.zeros((B, g["Hp"] // 2, g["Wp"] // 2 + 2, 16), dtype=torch.bfloat16,
+                                                        device=device) for g in tta_geometry(H, W, gs)[0][1:]]
+            self.members = [TTAPlan(m, B, H, W, device, compact_detect, conv_flags, det_out=self.pred, det_row_base=base,
+                                    stems=stems[gs]) for m, base, gs in zip(models, self.row_bases, gss)]
+            for i, p in enumerate(self.members):
+                self.steps.append((("layers", i, 0), lambda x, e=p.engines[0]: e.forward_s2d()))
+            for k in range(1, len(TTA_SCALES)):
+                for gs in sorted(set(gss)):
+                    idx = [i for i, g in enumerate(gss) if g == gs]
+                    self.steps.append((("resample", k, gs), lambda x, p=self.members[idx[0]], k=k: p.resample(x, k)))
+                    for i in idx:
+                        self.steps.append((("layers", i, k), lambda x, e=self.members[i].engines[k]: e.forward_s2d()))
+        for p, base in zip(self.members, self.row_bases):
+            assert p.pred is self.pred and base + p.rows_total <= self.rows_total
+        self.flops = sum(p.flops for p in self.members)
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        """x: [B,3,H,W] fp32 in [0,1] (or uint8 0..255) on this plan's device -> [B, rows_total, no] fp32 (or the compact
+        records), plan-owned, overwritten by the next call."""
+        _lib.require_cuda(x, "x")
+        if tuple(x.shape) != (self.B, 3, self.H, self.W):
+            raise RuntimeError(f"ensemble plan was built for {(self.B, 3, self.H, self.W)}, got {tuple(x.shape)}")
+        x = x.contiguous() if x.dtype == torch.uint8 else x.contiguous().float()
+        with torch.cuda.device(self.device):
+            for _, fn in self.steps:
+                fn(x)
+        return self.pred
+
+    def forward_s2d(self) -> torch.Tensor:
+        """Runs every member on an `x_s2d` the caller has already filled (scene tiles, letterboxed images) -> the shared
+        output, plan-owned as in forward().  Plain plans only: the augmented branches resample the image itself."""
+        if self.augment:
+            raise RuntimeError("forward_s2d runs the plain ensemble plan; test-time augmentation resamples the image in forward()")
+        with torch.cuda.device(self.device):
+            for _, fn in self.steps[1:]:
+                fn(None)
         return self.pred

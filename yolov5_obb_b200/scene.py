@@ -133,7 +133,8 @@ class SceneDetector:
     computes them.  Tiles run in batches of batch_size through one records plan; the last batch runs the full plan and the
     detections of its padding tiles are ignored.  pad=0.5 is val.py's rect-batching pad (1056^2 tiles for subsize 1024,
     1088^2 for a stride-64 P6 model: the size is rounded to the model's largest stride), pad=0.0 the unpadded tile of detect.py /
-    --task speed.  The model is one of the two families the engine plans: P5 (strides 8, 16, 32) or P6 (8, 16, 32, 64)."""
+    --task speed.  The model is one of the two families the engine plans: P5 (strides 8, 16, 32) or P6 (8, 16, 32, 64), or an
+    ensemble.Ensemble of them, whose stride is its largest member's (1088^2 tiles as soon as one member is a P6 model)."""
 
     def __init__(self, model, batch_size: int = 16, subsize: int = 1024, gap: int = 200, conf_thres: float = 0.01,
                  iou_thres: float = 0.4, max_det: int = 1500, merge_thresh: float = 0.2, pad: float = 0.5):

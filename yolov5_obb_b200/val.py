@@ -230,10 +230,15 @@ class Validator:
     Raw form: `im` may be the list of the batch's decoded source images (uint8 [h0, w0, 3] BGR arrays of any sizes) instead
     of the letterboxed tensor.  `shapes` then says where each one lands (letterbox.place_rect(...).shapes, the rect loader's
     entry); csrc/letterbox.cu resamples them as load_image_label + letterbox do and writes the plan's stem input, and
-    everything after the forward is the same.  targets stay in network-input pixels (Placement.map_labels)."""
+    everything after the forward is the same.  targets stay in network-input pixels (Placement.map_labels).
+    `model` may be an ensemble.Ensemble (val.py --weights a.pt b.pt); it has no validation loss."""
 
     def __init__(self, model, conf_thres: float = 0.01, iou_thres: float = 0.4, max_det: int = 1500, iouv=None,
                  augment: bool = False, compute_loss=None):
+        from .ensemble import Ensemble
+        if compute_loss is not None and isinstance(model, Ensemble):
+            # val.py run on an ensemble has no loss: train.py validates the single EMA model (val.py:198, compute_loss)
+            raise RuntimeError("the validation loss is defined for a single model, not an ensemble")
         self.model = model
         self.augment = bool(augment)   # val.py --augment: test-time augmentation (Model.detect_records(augment=True))
         self.device = _resolve(next(model.parameters()).device)
@@ -288,7 +293,8 @@ class Validator:
         return DetectRecords(eng.forward_s2d(), eng.nc), shape
 
     def __call__(self, batches) -> ValMetrics:
-        stats = ValStats(self.model.model[-1].nc, self.iouv.numel(), self.device)
+        nc = self.model.nc if hasattr(self.model, "nc") else self.model.model[-1].nc   # (an Ensemble has `nc`)
+        stats = ValStats(nc, self.iouv.numel(), self.device)
         pending = None
         self._loss, n_batches = torch.zeros(4, dtype=torch.float32, device=self.device), 0
         with torch.cuda.device(self.device):
