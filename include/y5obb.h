@@ -51,6 +51,10 @@ const char* y5obb_build_info(void);     /* "liby5obb sm_90a <date> <time>" */
                                        instead of the [batch, anchors, no] tensor (y5obb_conv_desc.det_decode = 2).  The theta
                                        index is the first maximum of the 180 theta LOGITS (= torch.max over their sigmoids,
                                        utils/general.py:822, whenever those are distinct) */
+#define Y5OBB_NMS_HALF 16            /* with Y5OBB_NMS_COMPACT_PRED only: the records come from an fp16 plan (Y5OBB_CONV_F16),
+                                       whose theta index is the first maximum of the fp16 sigmoids; conf = obj * cls is
+                                       rounded to fp16 as general.py:820 computes it on a half tensor.  The caller passes
+                                       conf_thres as torch compares a half tensor with a Python float: rounded to fp16 */
 
 /* Workspace needed for n_total boxes over n_images images with at most max_per_image boxes in any one
  * image (pass n_total if unknown). */
@@ -102,15 +106,16 @@ int y5obb_nms_obb_f32(const float* pred, int64_t batch, int64_t anchors, int no,
  * Replaces the cuDNN/ATen calls behind models/common.py:37-49 (Conv.forward_fuse = conv + folded-BN
  * bias + SiLU), :94-104 (Bottleneck residual), :267-274 (Concat, as a channel-offset store),
  * nn.Upsample(2x nearest) (models/yolov5*.yaml head) and models/yolo.py:49-81 (Detect).
- * Activations are NHWC bf16; a tensor argument is a channel SLICE of a wider buffer: `ptr` points at
+ * Activations are NHWC bf16, or fp16 with Y5OBB_CONV_F16 (the element type of input, weights, output and residual);
+ * a tensor argument is a channel SLICE of a wider buffer: `ptr` points at
  * the slice's first channel of pixel 0 and `*_pix_stride` is the element distance between pixels.
- * Weights are bf16 packed [KH*KW][cout_pad][cin_pad] (K-major), bias fp32 [cout_pad + 32]
+ * Weights are packed [KH*KW][cout_pad][cin_pad] (K-major) in that element type, bias fp32 [cout_pad + 32]
  * (the epilogue reads it in 32-wide chunks); the paddings and
  * the tile shape come from y5obb_conv_tiling so that host packing and kernel agree. */
 typedef struct y5obb_conv y5obb_conv_t;
 
-#define Y5OBB_CONV_MODE_CONV 0    /* bf16 NHWC output (+ optional residual / 2x up-sampled copy) */
-#define Y5OBB_CONV_MODE_DETECT 1  /* Detect head: fp32 [B, rows, no] output, optional sigmoid+decode */
+#define Y5OBB_CONV_MODE_CONV 0    /* bf16 (fp16) NHWC output (+ optional residual / 2x up-sampled copy) */
+#define Y5OBB_CONV_MODE_DETECT 1  /* Detect head: fp32 (fp16) [B, rows, no] output, optional sigmoid+decode; records are fp32 */
 
 #define Y5OBB_CONV_NO_ROWSHIFT 1   /* flags: force one TMA load per tap (debug / A-B comparison) */
 #define Y5OBB_CONV_NO_RESIDENT 2   /* flags: always stream the weight tiles */
@@ -124,9 +129,13 @@ typedef struct y5obb_conv y5obb_conv_t;
                                       the shared memory; debug / A-B comparison) */
 #define Y5OBB_CONV_DETECT_GENERIC 128  /* flags: compact Detect records (det_decode 2) through the shared epilogue instead of
                                       the records epilogue (default; bit-identical records); A-B comparison */
+#define Y5OBB_CONV_F16 256         /* flags: fp16 operands (wgmma .f16), fp16 output and residual (cvt.rn: overflow -> +-inf).
+                                      MODE_DETECT computes models/yolo.py:63-77 on a half tensor: fp16 logits, ATen's half
+                                      sigmoid, the decode rounded as torch rounds it, the theta index over the fp16 sigmoids,
+                                      and det_out holds fp16 rows (det_decode 0 / 1) or fp32 records of fp16 values (2) */
 
 typedef struct {
-  const void* in;            /* bf16 NHWC slice */
+  const void* in;            /* bf16 (fp16) NHWC slice */
   int64_t in_pix_stride;     /* elements between horizontally adjacent input pixels */
   int64_t in_row_stride;     /* elements between image rows (0 = Win * in_pix_stride) */
   int64_t in_img_stride;     /* elements between images     (0 = Hin * in_row_stride) */
@@ -137,13 +146,14 @@ typedef struct {
   int Cout, KH, KW, stride, pad_h, pad_w;
   int mode, act;             /* act: 0 = identity, 1 = SiLU */
   int flags;
-  void* out;                 /* bf16 NHWC slice (MODE_CONV) */
+  void* out;                 /* bf16 (fp16) NHWC slice (MODE_CONV) */
   int64_t out_pix_stride;
   const void* res;           /* optional residual slice added after the activation (Bottleneck.add) */
   int64_t res_pix_stride;
   void* out2x;               /* optional second destination receiving the 2x nearest up-sampled result */
   int64_t out2x_pix_stride;
-  float* det_out;            /* MODE_DETECT: fp32, row = b*det_rows_per_image + det_row_off + (a*H + h)*W + w */
+  float* det_out;            /* MODE_DETECT: fp32 (fp16 rows with Y5OBB_CONV_F16 and det_decode 0 / 1),
+                                row = b*det_rows_per_image + det_row_off + (a*H + h)*W + w */
   int64_t det_rows_per_image, det_row_off;
   int det_no;                /* outputs per anchor (nc + 5 + 180) */
   int det_decode;            /* 1: sigmoid + xy/wh decode (eval branch, yolo.py:71-74); 0: raw logits (train) */
@@ -195,6 +205,16 @@ int y5obb_scale_img_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int
 int y5obb_scale_img_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
                            int flip_lr, float pad_value, int pad_cols, void* stream);
 int y5obb_sppf_pool(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream);
+/* The same for the fp16 plans (Y5OBB_CONV_F16): an fp16 stem input holding the reference's half image - `x.half()` of an fp32
+ * image, fp16(u * (1 / 255)) of a uint8 one (val.py:187-188: `im.half()`, then ATen's half `/= 255`); the resample reads
+ * those fp16 values and rounds each output once to fp16; the pool works on an fp16 buffer. */
+int y5obb_stem_s2d_f16(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream);
+int y5obb_stem_s2d_u8_f16(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream);
+int y5obb_scale_img_s2d_f16(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                            int flip_lr, float pad_value, int pad_cols, void* stream);
+int y5obb_scale_img_s2d_u8_f16(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                               int flip_lr, float pad_value, int pad_cols, void* stream);
+int y5obb_sppf_pool_f16(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream);
 
 /* ---- loss ------------------------------------------------------------------------------------
  * Replaces utils/loss.py:122-192 (ComputeLoss.__call__), :194-275 (build_targets) and utils/metrics.py:201-236
@@ -242,17 +262,22 @@ int y5obb_loss_backward(const y5obb_loss_desc* desc, const float* grad_loss, voi
  * elements, or feat / w is not 16-byte aligned.  The workspace holds the obj logits (4 bytes per cell) and
  * nl * 5 * na * nt rows of no floats besides y5obb_loss_forward's own. */
 typedef struct {
-  const void* feat[Y5OBB_LOSS_MAX_LEVELS];   /* bf16 NHWC Detect input of level i (Detect.f[i]'s output) */
+  const void* feat[Y5OBB_LOSS_MAX_LEVELS];   /* bf16 (fp16) NHWC Detect input of level i (Detect.f[i]'s output) */
   int64_t pix_stride[Y5OBB_LOSS_MAX_LEVELS], row_stride[Y5OBB_LOSS_MAX_LEVELS],
       img_stride[Y5OBB_LOSS_MAX_LEVELS];     /* element strides of pixels, rows and images */
   int H[Y5OBB_LOSS_MAX_LEVELS], W[Y5OBB_LOSS_MAX_LEVELS], C[Y5OBB_LOSS_MAX_LEVELS];  /* feature shape; C % 8 == 0 */
-  const void* w[Y5OBB_LOSS_MAX_LEVELS];      /* bf16 [na * no, C]: Detect.m[i].weight */
+  const void* w[Y5OBB_LOSS_MAX_LEVELS];      /* bf16 (fp16) [na * no, C]: Detect.m[i].weight */
   const float* bias[Y5OBB_LOSS_MAX_LEVELS];  /* fp32 [na * no]:    Detect.m[i].bias */
 } y5obb_loss_head;
 
 size_t y5obb_loss_head_workspace_bytes(const y5obb_loss_desc* desc, const y5obb_loss_head* head);
 int y5obb_loss_forward_head(const y5obb_loss_desc* desc, const y5obb_loss_head* head, float* loss1, float* items4,
                             void* workspace, size_t workspace_bytes, void* stream);
+/* The same for an fp16 plan (Y5OBB_CONV_F16): feat and w are fp16, and each logit bias + sum_c feat * w is rounded to fp16
+ * before the loss reads it - the half Detect conv's output that val.py:198-199 widens with `x.float()`.  The workspace is
+ * y5obb_loss_head_workspace_bytes'. */
+int y5obb_loss_forward_head_f16(const y5obb_loss_desc* desc, const y5obb_loss_head* head, float* loss1, float* items4,
+                                void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- post-NMS geometry and CSL targets (one thread per box, fp32, separately rounded ops) -------
  * rbox2poly: utils/rboxs_utils.py:106-126 — [n,5] (cx,cy,l,s,theta) -> [n,8] corner coordinates.
@@ -461,6 +486,10 @@ typedef struct {
 } y5obb_letterbox_desc;      /* 64 bytes */
 int y5obb_letterbox_s2d_u8(const uint8_t* src, int64_t src_bytes, const void* desc_dev, const y5obb_letterbox_desc* desc_host,
                            int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16, int pad_cols, void* stream);
+/* the same into the fp16 stem input of an fp16 plan (Y5OBB_CONV_F16): each sample is fp16(u * (1 / 255)), as in
+ * y5obb_stem_s2d_u8_f16 */
+int y5obb_letterbox_s2d_u8_f16(const uint8_t* src, int64_t src_bytes, const void* desc_dev, const y5obb_letterbox_desc* desc_host,
+                               int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16, int pad_cols, void* stream);
 
 /* ---- whole-scene inference: tile input and tile-merge (DOTA scenes larger than one tile) --------------------------------
  * The reference's route (README.md:24-26): DOTA_devkit/ImgSplit_multi_process.py:226-273 cuts the scene into subsize^2 tiles
@@ -474,6 +503,9 @@ int y5obb_letterbox_s2d_u8(const uint8_t* src, int64_t src_bytes, const void* de
  * (up + y - border, left + x - border) in RGB order, or 0 beyond the scene.  The pad_cols columns are not written. */
 int y5obb_scene_tiles_s2d_u8(const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles, int subsize,
                              int size, int border, void* out_nhwc16, int pad_cols, void* stream);
+/* the same into the fp16 stem input of an fp16 plan (Y5OBB_CONV_F16), as y5obb_letterbox_s2d_u8_f16 */
+int y5obb_scene_tiles_s2d_u8_f16(const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles, int subsize,
+                                 int size, int border, void* out_nhwc16, int pad_cols, void* stream);
 /* y5obb_scene_merge_f64: rows7 [n_tiles, max_det, 7] + counts [n_tiles] = the packed output of y5obb_nms_obb_f32 for the tiles
  * (cx, cy, l, s, theta, conf, cls; counts[t] valid rows), origins2 as above -> out10 [K, 10] fp64 rows (class, score, x1 y1 ...
  * x4 y4), per class (ascending) in keep order, *n_out = K (out10 holds n_tiles * max_det rows).  Per row, as the reference's

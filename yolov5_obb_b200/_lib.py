@@ -46,6 +46,7 @@ PROTOTYPES = {
     "y5obb_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "y5obb_loss_head_workspace_bytes": (c_size_t, [c_void_p, c_void_p]),
     "y5obb_loss_forward_head": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "y5obb_loss_forward_head_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "y5obb_rbox2poly_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "y5obb_poly2hbb_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
     "y5obb_scale_polys_f32": (c_int, [c_void_p, c_int64, c_float, c_float, c_float, c_void_p]),
@@ -98,10 +99,19 @@ PROTOTYPES = {
     "y5obb_scale_img_s2d": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float, c_int, c_void_p]),
     "y5obb_scale_img_s2d_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float, c_int, c_void_p]),
     "y5obb_sppf_pool": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
+    "y5obb_stem_s2d_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "y5obb_stem_s2d_u8_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "y5obb_scale_img_s2d_f16": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float, c_int, c_void_p]),
+    "y5obb_scale_img_s2d_u8_f16": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float, c_int, c_void_p]),
+    "y5obb_sppf_pool_f16": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p]),
     "y5obb_scene_tiles_s2d_u8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                          c_void_p]),
+    "y5obb_scene_tiles_s2d_u8_f16": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                             c_int, c_void_p]),
     "y5obb_letterbox_s2d_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int,
                                        c_void_p]),
+    "y5obb_letterbox_s2d_u8_f16": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p,
+                                           c_int, c_void_p]),
     "y5obb_scene_merge_workspace_bytes": (c_size_t, [c_int64, c_int, c_int, c_void_p]),
     "y5obb_scene_merge_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_float, c_float, ctypes.c_double,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -129,6 +139,7 @@ NMS_STRICT_GT = 1
 NMS_DROP_SMALL = 2
 NMS_NO_CLASS_SPLIT = 4
 NMS_COMPACT_PRED = 8
+NMS_HALF = 16
 
 
 def lib() -> ctypes.CDLL:

@@ -1,6 +1,6 @@
 """Host-side handle for the wgmma implicit-GEMM convolution (csrc/conv_sm90.cu) behind the C ABI.
 
-A `Slice` names a channel range of an NHWC bf16 buffer; convs read and write slices, which is how
+A `Slice` names a channel range of an NHWC bf16 (or, in fp16 plans, fp16) buffer; convs read and write slices, which is how
 Concat (models/common.py:267-274) disappears: producers store at a channel offset.
 """
 import ctypes
@@ -36,13 +36,13 @@ class ConvDesc(ctypes.Structure):
 
 @dataclass
 class Slice:
-    """Channels [c_off, c_off + C) of an NHWC bf16 buffer [B, H, W, Ctot]."""
+    """Channels [c_off, c_off + C) of an NHWC bf16 or fp16 buffer [B, H, W, Ctot]."""
     buf: torch.Tensor
     c_off: int
     C: int
 
     def __post_init__(self):
-        assert self.buf.dtype == torch.bfloat16 and self.buf.dim() == 4 and self.buf.is_contiguous()
+        assert self.buf.dtype in (torch.bfloat16, torch.float16) and self.buf.dim() == 4 and self.buf.is_contiguous()
         assert 0 <= self.c_off and self.c_off + self.C <= self.buf.shape[3]
         assert self.c_off % 8 == 0 and self.buf.shape[3] % 8 == 0, "slices must start on 16-byte boundaries"
 
@@ -82,8 +82,10 @@ def tiling(cin: int, cout: int, mode: int = MODE_CONV, det_no: int = 0):
     return tuple(x.value for x in v)
 
 
-def pack_weights(w: torch.Tensor, bias: Optional[torch.Tensor], mode: int = MODE_CONV, det_no: int = 0):
-    """[Cout, Cin, KH, KW] fp32 (+ bias [Cout]) -> bf16 [KH*KW, cout_pad, cin_pad] K-major, fp32 bias [cout_pad + 32].
+def pack_weights(w: torch.Tensor, bias: Optional[torch.Tensor], mode: int = MODE_CONV, det_no: int = 0,
+                 dtype: torch.dtype = torch.bfloat16):
+    """[Cout, Cin, KH, KW] fp32 (+ bias [Cout]) -> `dtype` (bf16, or fp16 for the fp16 plans) [KH*KW, cout_pad, cin_pad]
+    K-major, fp32 bias [cout_pad + 32].
 
     Detect mode places anchor a's det_no rows at [a*block_n, a*block_n + det_no) so one N tile == one anchor.
     """
@@ -101,7 +103,7 @@ def pack_weights(w: torch.Tensor, bias: Optional[torch.Tensor], mode: int = MODE
         wp[:, :cout, :cin] = wt
         if bias is not None:
             bp[:cout] = bias.detach().float()
-    return wp.to(torch.bfloat16).contiguous(), bp.contiguous()
+    return wp.to(dtype).contiguous(), bp.contiguous()
 
 
 @dataclass
@@ -123,6 +125,7 @@ class WindowView:
 NO_ROWSHIFT, NO_RESIDENT, NO_PAIRW, BIAS_HALVED = 1, 2, 4, 8
 ONE_CTA = 64   # one CTA per SM for every instantiation (A/B comparison of the two-CTA plans)
 DETECT_GENERIC = 128   # compact Detect records through the shared epilogue (A/B comparison of the records epilogue)
+F16 = 256              # fp16 operands and outputs (Y5OBB_CONV_F16): the fp16 inference plans
 
 
 class Conv:

@@ -8,18 +8,24 @@
 //                      at channel offsets C, 2C, 3C of the same buffer (the torch.cat disappears).
 //   y5obb_scale_img_s2d  scale_img (bilinear resample, optional lr flip, pad) of a test-time-augmentation branch into
 //                      the same stem layout.
+// Each has an fp16 form (the *_f16 entry points) for the fp16 inference plans: the stem input is then the reference's half
+// image - `.half()` of an fp32 image, fp16(u * (1 / 255)) of a uint8 one (val.py:187-188: `im.half()`, then ATen's half
+// `/= 255`, a multiply by the fp32 reciprocal) - and the pooled maxima are fp16 (exact either way).
 // Algorithmic bytes: stem_s2d reads 12*H*W fp32 and writes H*W/4 * 32 B per image; scale_img_s2d reads the input once
 // (3*H*W elements) and writes Hp*Wp/4 * 32 B per image; sppf_pool reads H*W*C*2 and writes 3x that.
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <algorithm>
 
 #include "common.cuh"
+#include "stage.cuh"
 
 namespace y5obb {
 namespace {
 
-__global__ void k_stem_s2d(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, int B, int H, int W,
+template <typename E>
+__global__ void k_stem_s2d(const float* __restrict__ x, E* __restrict__ out, int B, int H, int W,
                            int pad_cols) {
   const int Ho = H >> 1, Wo = W >> 1;
   const long long total = (long long)B * Ho * Wo;
@@ -41,9 +47,7 @@ __global__ void k_stem_s2d(const float* __restrict__ x, __nv_bfloat16* __restric
     }
     v[12] = v[13] = v[14] = v[15] = 0.f;
     uint4 o[2];
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    pack16(v, out, o);
     // destination rows carry pad_cols zero pixels on each side (written once at allocation, never here)
     uint4* dst = reinterpret_cast<uint4*>(out + ((r * (Wo + 2 * pad_cols)) + wo + pad_cols) * 16);
     dst[0] = o[0];
@@ -53,7 +57,8 @@ __global__ void k_stem_s2d(const float* __restrict__ x, __nv_bfloat16* __restric
 
 // uint8 NCHW image: the caller-side `imgs.float() / 255` (train.py:299, val.py:187-188, detect.py:108-109)
 // folded into the same pass
-__global__ void k_stem_s2d_u8(const uint8_t* __restrict__ x, __nv_bfloat16* __restrict__ out, int B, int H, int W,
+template <typename E>
+__global__ void k_stem_s2d_u8(const uint8_t* __restrict__ x, E* __restrict__ out, int B, int H, int W,
                               int pad_cols) {
   const int Ho = H >> 1, Wo = W >> 1;
   const long long total = (long long)B * Ho * Wo;
@@ -68,16 +73,14 @@ __global__ void k_stem_s2d_u8(const uint8_t* __restrict__ x, __nv_bfloat16* __re
       const uint8_t* p = x + (((long long)b * 3 + c) * H + 2 * ho) * W + 2 * wo;
       const uchar2 top = *reinterpret_cast<const uchar2*>(p);
       const uchar2 bot = *reinterpret_cast<const uchar2*>(p + W);
-      v[0 * 3 + c] = (float)top.x / 255.0f;
-      v[1 * 3 + c] = (float)top.y / 255.0f;
-      v[2 * 3 + c] = (float)bot.x / 255.0f;
-      v[3 * 3 + c] = (float)bot.y / 255.0f;
+      v[0 * 3 + c] = u8_value(top.x, out);
+      v[1 * 3 + c] = u8_value(top.y, out);
+      v[2 * 3 + c] = u8_value(bot.x, out);
+      v[3 * 3 + c] = u8_value(bot.y, out);
     }
     v[12] = v[13] = v[14] = v[15] = 0.f;
     uint4 o[2];
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    pack16(v, out, o);
     // destination rows carry pad_cols zero pixels on each side (written once at allocation, never here)
     uint4* dst = reinterpret_cast<uint4*>(out + ((r * (Wo + 2 * pad_cols)) + wo + pad_cols) * 16);
     dst[0] = o[0];
@@ -92,8 +95,12 @@ __global__ void k_stem_s2d_u8(const uint8_t* __restrict__ x, __nv_bfloat16* __re
 //   val = fma(h0l, fma(w0l, x00, w1l * x01), h1l * fma(w0l, x10, w1l * x11))
 // (the second product of each sum is the plain multiply: FMUL + FFMA pairs in the sm_90 SASS torch ships).
 // Pixels at or beyond (h, w) hold F.pad's value.  The left-right flip reads column W - 1 - xs of x.
-__device__ __forceinline__ float ld_px(const float* p, long long i) { return p[i]; }
-__device__ __forceinline__ float ld_px(const uint8_t* p, long long i) { return (float)p[i] / 255.0f; }
+__device__ __forceinline__ float ld_px(const float* p, long long i, __nv_bfloat16*) { return p[i]; }
+__device__ __forceinline__ float ld_px(const uint8_t* p, long long i, __nv_bfloat16* e) { return u8_value(p[i], e); }
+// fp16 plans: scale_img of the half image (upsample_bilinear2d_out_frame<Half, float>: fp16 inputs, fp32 arithmetic, one
+// rounding to fp16 at the store)
+__device__ __forceinline__ float ld_px(const float* p, long long i, __half*) { return __half2float(__float2half_rn(p[i])); }
+__device__ __forceinline__ float ld_px(const uint8_t* p, long long i, __half* e) { return u8_value(p[i], e); }
 
 __device__ __forceinline__ void bil_src(float scale, int dst, int in, int& i0, int& i1, float& l0, float& l1) {
   float s = __fmaf_rn(scale, (float)dst + 0.5f, -0.5f);
@@ -104,8 +111,8 @@ __device__ __forceinline__ void bil_src(float scale, int dst, int in, int& i0, i
   l0 = __fsub_rn(1.0f, l1);
 }
 
-template <typename T>
-__global__ void k_scale_img_s2d(const T* __restrict__ x, __nv_bfloat16* __restrict__ out, int B, int H, int W, int h, int w,
+template <typename T, typename E>
+__global__ void k_scale_img_s2d(const T* __restrict__ x, E* __restrict__ out, int B, int H, int W, int h, int w,
                                 int Hp, int Wp, int flip, float pad_value, float rh, float rw, int pad_cols) {
   const int Ho = Hp >> 1, Wo = Wp >> 1;
   const long long total = (long long)B * Ho * Wo;
@@ -140,24 +147,22 @@ __global__ void k_scale_img_s2d(const T* __restrict__ x, __nv_bfloat16* __restri
         for (int c = 0; c < 3; ++c) {
           const T* p = x + ((long long)b * 3 + c) * H * W;
           const long long r0 = (long long)y0 * W, r1 = (long long)y1 * W;
-          const float a = __fmaf_rn(wl0, ld_px(p, r0 + x0), __fmul_rn(wl1, ld_px(p, r0 + x1)));
-          const float e = __fmaf_rn(wl0, ld_px(p, r1 + x0), __fmul_rn(wl1, ld_px(p, r1 + x1)));
+          const float a = __fmaf_rn(wl0, ld_px(p, r0 + x0, out), __fmul_rn(wl1, ld_px(p, r0 + x1, out)));
+          const float e = __fmaf_rn(wl0, ld_px(p, r1 + x0, out), __fmul_rn(wl1, ld_px(p, r1 + x1, out)));
           d[c] = __fmaf_rn(hl0, a, __fmul_rn(hl1, e));
         }
       }
     }
     v[12] = v[13] = v[14] = v[15] = 0.f;
     uint4 o[2];
-    __nv_bfloat162* hv = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) hv[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    pack16(v, out, o);
     uint4* dst = reinterpret_cast<uint4*>(out + ((r * (Wo + 2 * pad_cols)) + wo + pad_cols) * 16);
     dst[0] = o[0];
     dst[1] = o[1];
   }
 }
 
-template <typename T>
+template <typename T, typename E>
 int scale_img_s2d(const T* x, void* out, int B, int H, int W, int h, int w, int Hp, int Wp, int flip, float pad_value,
                   int pad_cols, void* stream) {
   if (!x || !out || B <= 0 || H <= 0 || W <= 0 || h <= 0 || w <= 0 || Hp <= 0 || Wp <= 0 || (Hp & 1) || (Wp & 1) ||
@@ -168,24 +173,29 @@ int scale_img_s2d(const T* x, void* out, int B, int H, int W, int h, int w, int 
   const float rh = (float)H / (float)h, rw = (float)W / (float)w;
   const long long total = (long long)B * (Hp / 2) * (Wp / 2);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  k_scale_img_s2d<T><<<grid, 256, 0, (cudaStream_t)stream>>>(x, static_cast<__nv_bfloat16*>(out), B, H, W, h, w, Hp, Wp,
-                                                             flip ? 1 : 0, pad_value, rh, rw, pad_cols);
+  k_scale_img_s2d<T, E><<<grid, 256, 0, (cudaStream_t)stream>>>(x, static_cast<E*>(out), B, H, W, h, w, Hp, Wp,
+                                                                flip ? 1 : 0, pad_value, rh, rw, pad_cols);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
 }
 
+template <typename E2>
 __device__ __forceinline__ void vmax8(uint4& a, const uint4& b) {
-  __nv_bfloat162* x = reinterpret_cast<__nv_bfloat162*>(&a);
-  const __nv_bfloat162* y = reinterpret_cast<const __nv_bfloat162*>(&b);
+  E2* x = reinterpret_cast<E2*>(&a);
+  const E2* y = reinterpret_cast<const E2*>(&b);
 #pragma unroll
   for (int i = 0; i < 4; ++i) x[i] = __hmax2(x[i], y[i]);
 }
+template <typename E> struct Pair;
+template <> struct Pair<__nv_bfloat16> { using T = __nv_bfloat162; static constexpr uint32_t NINF = 0xFF80FF80u; };
+template <> struct Pair<__half> { using T = __half2; static constexpr uint32_t NINF = 0xFC00FC00u; };
 
 // One CTA = one image x 8 channels x one 32x32 spatial tile (+6 halo).  Separable: a horizontal pass builds the
 // 5/9/13-wide row maxima in shared memory, a vertical pass the 5/9/13-tall column maxima of those (max-pool pads
 // with -inf, so clipped windows are exact).  13 + 27 shared-memory reads per pixel instead of 169 global ones.
 constexpr int PT = 32, PH = 6, PIN = PT + 2 * PH;
-__global__ void __launch_bounds__(256) k_sppf_pool(__nv_bfloat16* __restrict__ buf, long long pix_stride, int B, int H,
+template <typename E>
+__global__ void __launch_bounds__(256) k_sppf_pool(E* __restrict__ buf, long long pix_stride, int B, int H,
                                                     int W, int C, int tiles_w, int tiles_h) {
   extern __shared__ __align__(16) uint4 sm[];
   uint4* in = sm;                       // [PIN][PIN]
@@ -201,8 +211,9 @@ __global__ void __launch_bounds__(256) k_sppf_pool(__nv_bfloat16* __restrict__ b
   const int th = bid % tiles_h;
   const int b = bid / tiles_h;
   const int h0 = th * PT, w0 = tw * PT;
-  const uint4 ninf = make_uint4(0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u, 0xFF80FF80u);
-  const __nv_bfloat16* base = buf + (long long)b * H * W * pix_stride + cv * 8;
+  constexpr uint32_t NI2 = Pair<E>::NINF;
+  const uint4 ninf = make_uint4(NI2, NI2, NI2, NI2);
+  const E* base = buf + (long long)b * H * W * pix_stride + cv * 8;
   for (int i = threadIdx.x; i < PIN * PIN; i += 256) {
     const int y = i / PIN, x = i - y * PIN;
     const int hh = h0 + y - PH, ww = w0 + x - PH;
@@ -215,20 +226,20 @@ __global__ void __launch_bounds__(256) k_sppf_pool(__nv_bfloat16* __restrict__ b
     const int y = i / PT, x = i - y * PT;
     const uint4* row = in + y * PIN + x + PH;
     uint4 a5 = row[0];
-    vmax8(a5, row[-1]);
-    vmax8(a5, row[1]);
-    vmax8(a5, row[-2]);
-    vmax8(a5, row[2]);
+    vmax8<typename Pair<E>::T>(a5, row[-1]);
+    vmax8<typename Pair<E>::T>(a5, row[1]);
+    vmax8<typename Pair<E>::T>(a5, row[-2]);
+    vmax8<typename Pair<E>::T>(a5, row[2]);
     uint4 a9 = a5;
-    vmax8(a9, row[-3]);
-    vmax8(a9, row[3]);
-    vmax8(a9, row[-4]);
-    vmax8(a9, row[4]);
+    vmax8<typename Pair<E>::T>(a9, row[-3]);
+    vmax8<typename Pair<E>::T>(a9, row[3]);
+    vmax8<typename Pair<E>::T>(a9, row[-4]);
+    vmax8<typename Pair<E>::T>(a9, row[4]);
     uint4 a13 = a9;
-    vmax8(a13, row[-5]);
-    vmax8(a13, row[5]);
-    vmax8(a13, row[-6]);
-    vmax8(a13, row[6]);
+    vmax8<typename Pair<E>::T>(a13, row[-5]);
+    vmax8<typename Pair<E>::T>(a13, row[5]);
+    vmax8<typename Pair<E>::T>(a13, row[-6]);
+    vmax8<typename Pair<E>::T>(a13, row[6]);
     r5[i] = a5;
     r9[i] = a9;
     r13[i] = a13;
@@ -241,24 +252,66 @@ __global__ void __launch_bounds__(256) k_sppf_pool(__nv_bfloat16* __restrict__ b
     const int c = (y + PH) * PT + x;
     uint4 m5 = r5[c];
     for (int d = 1; d <= 2; ++d) {
-      vmax8(m5, r5[c - d * PT]);
-      vmax8(m5, r5[c + d * PT]);
+      vmax8<typename Pair<E>::T>(m5, r5[c - d * PT]);
+      vmax8<typename Pair<E>::T>(m5, r5[c + d * PT]);
     }
     uint4 m9 = r9[c];
     for (int d = 1; d <= 4; ++d) {
-      vmax8(m9, r9[c - d * PT]);
-      vmax8(m9, r9[c + d * PT]);
+      vmax8<typename Pair<E>::T>(m9, r9[c - d * PT]);
+      vmax8<typename Pair<E>::T>(m9, r9[c + d * PT]);
     }
     uint4 m13 = r13[c];
     for (int d = 1; d <= 6; ++d) {
-      vmax8(m13, r13[c - d * PT]);
-      vmax8(m13, r13[c + d * PT]);
+      vmax8<typename Pair<E>::T>(m13, r13[c - d * PT]);
+      vmax8<typename Pair<E>::T>(m13, r13[c + d * PT]);
     }
-    __nv_bfloat16* o = buf + (((long long)b * H + hh) * W + ww) * pix_stride + cv * 8;
+    E* o = buf + (((long long)b * H + hh) * W + ww) * pix_stride + cv * 8;
     *reinterpret_cast<uint4*>(o + C) = m5;
     *reinterpret_cast<uint4*>(o + 2 * C) = m9;
     *reinterpret_cast<uint4*>(o + 3 * C) = m13;
   }
+}
+
+template <typename E>
+int stem_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream) {
+  if (!x_nchw || !out_nhwc16 || B <= 0 || H <= 0 || W <= 0 || (H & 1) || (W & 1) || pad_cols < 0) return Y5OBB_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(x_nchw) & 7) || (reinterpret_cast<uintptr_t>(out_nhwc16) & 15)) return Y5OBB_EINVAL;
+  const long long total = (long long)B * (H / 2) * (W / 2);
+  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
+  k_stem_s2d<E><<<grid, 256, 0, (cudaStream_t)stream>>>(x_nchw, static_cast<E*>(out_nhwc16), B, H, W, pad_cols);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+template <typename E>
+int stem_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream) {
+  if (!x_nchw || !out_nhwc16 || B <= 0 || H <= 0 || W <= 0 || (H & 1) || (W & 1) || pad_cols < 0) return Y5OBB_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(x_nchw) & 1) || (reinterpret_cast<uintptr_t>(out_nhwc16) & 15)) return Y5OBB_EINVAL;
+  const long long total = (long long)B * (H / 2) * (W / 2);
+  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
+  k_stem_s2d_u8<E><<<grid, 256, 0, (cudaStream_t)stream>>>(x_nchw, static_cast<E*>(out_nhwc16), B, H, W, pad_cols);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+template <typename E>
+int sppf_pool(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream) {
+  if (!buf || B <= 0 || H <= 0 || W <= 0 || C <= 0 || (C & 7) || (pix_stride & 7) || pix_stride < 4 * (int64_t)C)
+    return Y5OBB_EINVAL;
+  if (reinterpret_cast<uintptr_t>(buf) & 15) return Y5OBB_EINVAL;
+  const int tiles_w = (W + PT - 1) / PT, tiles_h = (H + PT - 1) / PT;
+  const long long grid = (long long)B * (C / 8) * tiles_w * tiles_h;
+  if (grid > 0x7FFFFFFFll) return Y5OBB_EINVAL;
+  const size_t smem = (size_t)(PIN * PIN + 3 * PIN * PT) * sizeof(uint4);
+  static bool attr_set = false;
+  if (!attr_set) {
+    Y5_CUDA(cudaFuncSetAttribute(k_sppf_pool<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  k_sppf_pool<E><<<(unsigned)grid, 256, smem, (cudaStream_t)stream>>>(static_cast<E*>(buf), pix_stride, B, H, W, C, tiles_w,
+                                                                     tiles_h);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
 }
 
 }  // namespace
@@ -269,52 +322,48 @@ using namespace y5obb;
 extern "C" {
 
 int y5obb_stem_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream) {
-  if (!x_nchw || !out_nhwc16 || B <= 0 || H <= 0 || W <= 0 || (H & 1) || (W & 1) || pad_cols < 0) return Y5OBB_EINVAL;
-  if ((reinterpret_cast<uintptr_t>(x_nchw) & 7) || (reinterpret_cast<uintptr_t>(out_nhwc16) & 15)) return Y5OBB_EINVAL;
-  const long long total = (long long)B * (H / 2) * (W / 2);
-  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  k_stem_s2d<<<grid, 256, 0, (cudaStream_t)stream>>>(x_nchw, static_cast<__nv_bfloat16*>(out_nhwc16), B, H, W, pad_cols);
-  Y5_LAUNCH_CHECK();
-  return Y5OBB_OK;
+  return stem_s2d<__nv_bfloat16>(x_nchw, out_nhwc16, B, H, W, pad_cols, stream);
 }
 
 int y5obb_stem_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream) {
-  if (!x_nchw || !out_nhwc16 || B <= 0 || H <= 0 || W <= 0 || (H & 1) || (W & 1) || pad_cols < 0) return Y5OBB_EINVAL;
-  if ((reinterpret_cast<uintptr_t>(x_nchw) & 1) || (reinterpret_cast<uintptr_t>(out_nhwc16) & 15)) return Y5OBB_EINVAL;
-  const long long total = (long long)B * (H / 2) * (W / 2);
-  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  k_stem_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(x_nchw, static_cast<__nv_bfloat16*>(out_nhwc16), B, H, W, pad_cols);
-  Y5_LAUNCH_CHECK();
-  return Y5OBB_OK;
+  return stem_s2d_u8<__nv_bfloat16>(x_nchw, out_nhwc16, B, H, W, pad_cols, stream);
+}
+
+int y5obb_stem_s2d_f16(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream) {
+  return stem_s2d<__half>(x_nchw, out_nhwc16, B, H, W, pad_cols, stream);
+}
+
+int y5obb_stem_s2d_u8_f16(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int pad_cols, void* stream) {
+  return stem_s2d_u8<__half>(x_nchw, out_nhwc16, B, H, W, pad_cols, stream);
 }
 
 int y5obb_scale_img_s2d(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
                         int flip_lr, float pad_value, int pad_cols, void* stream) {
-  return scale_img_s2d(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
+  return scale_img_s2d<float, __nv_bfloat16>(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
 }
 
 int y5obb_scale_img_s2d_u8(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
                            int flip_lr, float pad_value, int pad_cols, void* stream) {
-  return scale_img_s2d(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
+  return scale_img_s2d<uint8_t, __nv_bfloat16>(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols,
+                                               stream);
+}
+
+int y5obb_scale_img_s2d_f16(const float* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                            int flip_lr, float pad_value, int pad_cols, void* stream) {
+  return scale_img_s2d<float, __half>(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
+}
+
+int y5obb_scale_img_s2d_u8_f16(const uint8_t* x_nchw, void* out_nhwc16, int B, int H, int W, int h, int w, int Hp, int Wp,
+                               int flip_lr, float pad_value, int pad_cols, void* stream) {
+  return scale_img_s2d<uint8_t, __half>(x_nchw, out_nhwc16, B, H, W, h, w, Hp, Wp, flip_lr, pad_value, pad_cols, stream);
 }
 
 int y5obb_sppf_pool(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream) {
-  if (!buf || B <= 0 || H <= 0 || W <= 0 || C <= 0 || (C & 7) || (pix_stride & 7) || pix_stride < 4 * (int64_t)C)
-    return Y5OBB_EINVAL;
-  if (reinterpret_cast<uintptr_t>(buf) & 15) return Y5OBB_EINVAL;
-  const int tiles_w = (W + PT - 1) / PT, tiles_h = (H + PT - 1) / PT;
-  const long long grid = (long long)B * (C / 8) * tiles_w * tiles_h;
-  if (grid > 0x7FFFFFFFll) return Y5OBB_EINVAL;
-  const size_t smem = (size_t)(PIN * PIN + 3 * PIN * PT) * sizeof(uint4);
-  static bool attr_set = false;
-  if (!attr_set) {
-    Y5_CUDA(cudaFuncSetAttribute(k_sppf_pool, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  k_sppf_pool<<<(unsigned)grid, 256, smem, (cudaStream_t)stream>>>(static_cast<__nv_bfloat16*>(buf), pix_stride, B, H, W,
-                                                                  C, tiles_w, tiles_h);
-  Y5_LAUNCH_CHECK();
-  return Y5OBB_OK;
+  return sppf_pool<__nv_bfloat16>(buf, pix_stride, B, H, W, C, stream);
+}
+
+int y5obb_sppf_pool_f16(void* buf, int64_t pix_stride, int B, int H, int W, int C, void* stream) {
+  return sppf_pool<__half>(buf, pix_stride, B, H, W, C, stream);
 }
 
 }  // extern "C"

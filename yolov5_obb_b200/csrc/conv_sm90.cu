@@ -1,4 +1,4 @@
-// Implicit-GEMM NHWC bf16 convolution for sm_90a: TMA -> shared memory -> wgmma (fp32 accumulators in registers) ->
+// Implicit-GEMM NHWC bf16 (or fp16, F16 / Y5OBB_CONV_F16) convolution for sm_90a: TMA -> shared memory -> wgmma (fp32 accumulators in registers) ->
 // fused epilogue (folded-BN bias, SiLU, residual add, concat-offset store, 2x nearest up-sample copy, or the Detect
 // head's permute + sigmoid + grid/anchor decode).
 //
@@ -22,6 +22,7 @@
 // (algorithmic bytes = input pixels*Cin*2 + output pixels*Cout*2 [+ residual] per image).
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <algorithm>
 #include <cstdlib>
@@ -154,6 +155,26 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// fp16 plans (F16, Y5OBB_CONV_F16): cvt.rn.f16x2.f32 - overflow rounds to +-inf, as torch's half conversion does
+__device__ __forceinline__ uint32_t pack_f16(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <bool F16>
+__device__ __forceinline__ uint32_t pack_elem2(float a, float b) {
+  if constexpr (F16) return pack_f16(a, b);
+  else return pack_bf16(a, b);
+}
+template <bool F16>
+__device__ __forceinline__ float2 unpack_elem2(uint32_t v) {
+  if constexpr (F16) return __half22float2(*reinterpret_cast<const __half2*>(&v));
+  else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v));
+}
+// the fp32 value of x rounded to fp16
+__device__ __forceinline__ float r16(float x) { return __half2float(__float2half_rn(x)); }
+// ATen's half sigmoid (fp32 opmath, IEEE division, one rounding to fp16) of the fp16 logit l
+__device__ __forceinline__ float sigmoid16(float l) { return r16(__fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-l)))); }
+
 __device__ __forceinline__ uint64_t desc_from(uint32_t lo, uint32_t hi) {
   uint64_t d;
   asm volatile("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
@@ -265,12 +286,12 @@ __device__ __forceinline__ uint32_t stg_chunk(uint32_t i) { return (i ^ ((i >> 3
 // MODE_CONV.  The warp owns 16 pixel rows (row0 .. row0 + 15 of the tile).  wgmma's accumulator layout gives thread
 // `lane` the rows row0 + lane / 4 (+ 8) and the column pairs 8 j + 2 (lane % 4) (+ 1): for each pair of 8-column groups,
 // exactly the four 8 x 8 matrices of one stmatrix.x4.  Per 64-column block: bias (+ SiLU) in registers, the residual
-// (RES) added in fp32 in registers, one rounding to bf16, the block staged as [16 rows][64] bf16 by stmatrix, and 16-byte
+// (RES) added in fp32 in registers, one rounding to bf16 (fp16 when F16), the block staged as [16 rows][64] bf16 by stmatrix, and 16-byte
 // stores per pixel.  RES: rpf holds the residual of the first StoreVecs<NI>::PREFETCH blocks in the accumulator layout,
 // loaded when the tile started; a later block's residual is copied by cp.async into the staging area's second half in the
 // store layout and comes back in the accumulator layout by ldmatrix.  The probe's phases: CP_STAGED the activation and
 // the staging, CP_RES the wait for the residual, CP_STORED the stores.
-template <int NI, bool RES>
+template <int NI, bool RES, bool F16>
 __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg, const float* bias_s,
                                          const uint32_t (&rpf)[StoreVecs<NI>::DIM][StoreVecs<NI>::FRAG], int row0,
                                          int lane, int ti) {
@@ -352,11 +373,11 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
         for (int m = 0; m < 4; ++m) {
           float f0 = acc[4 * (j0 + m / 2) + 2 * (m % 2)], f1 = acc[4 * (j0 + m / 2) + 2 * (m % 2) + 1];
           if constexpr (RES) {
-            const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rb[m]));
+            const float2 g = unpack_elem2<F16>(rb[m]);
             f0 += g.x;
             f1 += g.y;
           }
-          o[m] = pack_bf16(f0, f1);
+          o[m] = pack_elem2<F16>(f0, f1);
         }
         ptx::stmatrix_x4(out_s + stg_chunk(mat + 2 * jp), o);
       }
@@ -399,9 +420,28 @@ __device__ __forceinline__ void epilogue(const ConvK& p, const TileCoord& c, flo
   }
 }
 
+// F16 decode of the first four columns (f: their fp16 sigmoids) of anchor a at grid cell (gx, gy), as models/yolo.py:72-73
+// computes it on a half y: xy = fp16((fp16(2 y - 0.5) + grid) * stride), wh = fp16(fp16((2 y)^2) * anchor_grid), and
+// _descale_pred's half `/= s` (a multiply by the fp32 1/s) and `W - x`.  2 y, 2 y - 0.5 and (2 y)^2 are exact in fp32.
+__device__ __forceinline__ void decode16(const ConvK& p, float (&f)[4], float gx, float gy, int a) {
+  f[0] = r16(__fmul_rn(__fadd_rn(r16(__fsub_rn(2.0f * f[0], 0.5f)), gx), p.det_stride));
+  f[1] = r16(__fmul_rn(__fadd_rn(r16(__fsub_rn(2.0f * f[1], 0.5f)), gy), p.det_stride));
+  f[2] = r16(__fmul_rn(r16(__fmul_rn(2.0f * f[2], 2.0f * f[2])), p.det_anchor[2 * a]));
+  f[3] = r16(__fmul_rn(r16(__fmul_rn(2.0f * f[3], 2.0f * f[3])), p.det_anchor[2 * a + 1]));
+  if (p.det_descale) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) f[k] = r16(__fmul_rn(f[k], p.det_inv_scale));
+    if (p.det_flip_w > 0.0f) f[0] = r16(__fsub_rn(p.det_flip_w, f[0]));
+  }
+}
+
 // MODE_DETECT through the shared epilogue (every Detect launch that is not epilogue_records').  Each 64-column block is
 // activated in registers, staged through shared memory as [16 rows][64] fp32 and leaves as fp32 rows.
-template <int NI>
+// F16: models/yolo.py:63-77 on a half tensor, operation by operation.  Each logit is rounded to fp16 (the conv's output),
+// sigmoid16 activates it, the decode rounds to fp16 where torch stores a half tensor (grid, stride and anchor_grid are
+// fp32, so their add and multiplies run in fp32 first), the theta index is the first maximum of the 180 fp16 sigmoids,
+// and rows other than records leave as fp16.
+template <int NI, bool F16>
 __device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], float* stg,
                                                 const float* bias_s, int row0, int lane, int ti) {
   const int q = lane & 3, r = lane >> 2;
@@ -422,7 +462,8 @@ __device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord&
         if (col >= nfix && col < p.det_no) {
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
-            const float v = acc[4 * j + 2 * i + k] + bias[col];
+            float v = acc[4 * j + 2 * i + k] + bias[col];
+            if constexpr (F16) v = sigmoid16(r16(v));
             if (v > best[i]) {
               best[i] = v;
               bk[i] = col - nfix;
@@ -467,6 +508,10 @@ __device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord&
             v0 += b0;
             v1 += b1;
           }
+          if constexpr (F16) {
+            v0 = r16(v0);
+            v1 = r16(v1);
+          }
           *reinterpret_cast<float2*>(stg + (r + 8 * i) * PITCH + (col - cb)) = make_float2(v0, v1);
         }
       }
@@ -488,8 +533,10 @@ __device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord&
       float f[4] = {x.x, x.y, x.z, x.w};
       if (p.det_decode) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) f[k] = sigmoid_fast(f[k]);
-        if (col == 0) {  // xy, wh (models/yolo.py)
+        for (int k = 0; k < 4; ++k) f[k] = F16 ? sigmoid16(f[k]) : sigmoid_fast(f[k]);
+        if (F16 && col == 0) {
+          decode16(p, f, (float)w, (float)h, a);
+        } else if (col == 0) {  // xy, wh (models/yolo.py)
           f[0] = (f[0] * 2.0f - 0.5f + (float)w) * p.det_stride;
           f[1] = (f[1] * 2.0f - 0.5f + (float)h) * p.det_stride;
           f[2] = (f[2] * 2.0f) * (f[2] * 2.0f) * p.det_anchor[2 * a];
@@ -508,6 +555,17 @@ __device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord&
         }
       }
       const long long orow = (long long)c.b * p.det_rows_per_image + p.det_row_off + ((long long)a * p.Hout + h) * p.Wout + w;
+      if (F16 && p.det_decode != 2) {  // fp16 rows: 8-byte vectors when rows are 4-aligned, element stores otherwise
+        __half* dst = reinterpret_cast<__half*>(p.det_out) + orow * rw + col;
+        if (!(rw & 3)) {
+          *reinterpret_cast<uint2*>(dst) = make_uint2(pack_f16(f[0], f[1]), pack_f16(f[2], f[3]));
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (col + k < ncols) dst[k] = __float2half_rn(f[k]);
+        }
+        continue;
+      }
       float* dst = p.det_out + orow * rw + col;
       if (!(rw & 3)) {
         *reinterpret_cast<float4*>(dst) = make_float4(f[0], f[1], f[2], f[3]);
@@ -536,7 +594,9 @@ __device__ __forceinline__ void epilogue_detect(const ConvK& p, const TileCoord&
 // consecutive pixels of one image row (all 16 when the tile spans whole image rows, Wt == Wout) are consecutive records of
 // [B, A, rec_w], so each run of them leaves in one cp.async.bulk store.  The store reads the staging buffer asynchronously;
 // the next tile's epilogue waits for that read before it writes the buffer again, so the store overlaps the next tile's MMAs.
-template <int NI>
+// F16: the record of epilogue_detect<NI, true> - fp16 logits, sigmoid16, decode16, and the first maximum of the 180 fp16
+// sigmoids, which rounding can tie where the logits differ.  The -inf of a non-theta column stays -inf instead.
+template <int NI, bool F16>
 __device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord& c, float (&acc)[NI / 2], const float* bt_s,
                                                  float* stg, const float* bias_s, int row0, int lane, int ti) {
   const int q = lane & 3, r = lane >> 2;
@@ -554,7 +614,9 @@ __device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord
     for (int k = 0; k < 2; ++k)
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const float v = acc[4 * j + 2 * i + k] + (k ? bt.y : bt.x);
+        const float b = k ? bt.y : bt.x;
+        float v = acc[4 * j + 2 * i + k] + b;
+        if constexpr (F16) v = b == -INFINITY ? -INFINITY : sigmoid16(r16(v));
         const bool take = v > best[i];
         best[i] = take ? v : best[i];
         bk[i] = take ? 8 * j + 2 * q + k : bk[i];
@@ -594,8 +656,20 @@ __device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord
     const float2 b = col < nfix ? ptx::ld_shared_v2(ptx::smem_u32(bias + col)) : make_float2(0.0f, 0.0f);
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      float f0 = sigmoid_fast(acc[4 * j + 2 * i] + b.x), f1 = sigmoid_fast(acc[4 * j + 2 * i + 1] + b.y);
-      if (j == 0 && q < 2) {  // xy, wh (models/yolo.py)
+      float f0, f1;
+      if constexpr (F16) {
+        f0 = sigmoid16(r16(acc[4 * j + 2 * i] + b.x));
+        f1 = sigmoid16(r16(acc[4 * j + 2 * i + 1] + b.y));
+      } else {
+        f0 = sigmoid_fast(acc[4 * j + 2 * i] + b.x);
+        f1 = sigmoid_fast(acc[4 * j + 2 * i + 1] + b.y);
+      }
+      if (F16 && j == 0 && q < 2) {  // decode16's columns 0, 1 (q = 0) or 2, 3 (q = 1)
+        float f[4] = {f0, f1, f0, f1};
+        decode16(p, f, px[i], py[i], a);
+        f0 = q == 0 ? f[0] : f[2];
+        f1 = q == 0 ? f[1] : f[3];
+      } else if (j == 0 && q < 2) {  // xy, wh (models/yolo.py)
         if (q == 0) {
           f0 = (f0 * 2.0f - 0.5f + px[i]) * p.det_stride;
           f1 = (f1 * 2.0f - 0.5f + py[i]) * p.det_stride;
@@ -642,7 +716,7 @@ __device__ __forceinline__ void epilogue_records(const ConvK& p, const TileCoord
 // RECORDS: the Detect head with compact records (epilogue_records); otherwise epilogue_detect for the other Detect launches
 // and epilogue<NI, RES> for every conv.  RES: a MODE_CONV launch with a residual, whose residual vectors are loaded when
 // each tile starts.
-template <int NI, bool RECORDS, bool RES = false>
+template <int NI, bool RECORDS, bool RES = false, bool F16 = false>
 __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_kernel(const __grid_constant__ ConvK p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
@@ -797,7 +871,7 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
         const int nk = last ? nk_last : nk_full;
         for (int u = 0; u < ksub; ++u)
           for (int j = 0; j < nk; ++j) {
-            ptx::Wgmma<NI>::template mma<0, 0>(acc, desc_from(a_lo + (uint32_t)u * a_step + 2u * j, hi),
+            ptx::Wgmma<NI>::template mma<0, 0, F16>(acc, desc_from(a_lo + (uint32_t)u * a_step + 2u * j, hi),
                                                desc_from(b_lo + (uint32_t)u * b_step + 2u * j, hi), scale_d);
             scale_d = 1u;
           }
@@ -838,11 +912,11 @@ __global__ void __launch_bounds__(NUM_THREADS, Occupancy<NI>::CTAS) conv_wgmma_k
         asm volatile("bar.sync 1, %0;" ::"n"(32 * CONSUMER_WARPS) : "memory");
         bt_nt = c.nt;
       }
-      epilogue_records<NI>(p, c, acc, bt_s, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
+      epilogue_records<NI, F16>(p, c, acc, bt_s, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
     } else if (p.mode == MODE_DETECT) {
-      if constexpr (!RES) epilogue_detect<NI>(p, c, acc, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
+      if constexpr (!RES) epilogue_detect<NI, F16>(p, c, acc, stg, bias_s, wg * 64 + (warp & 3) * 16, lane, ti);
     } else {
-      epilogue<NI, RES>(p, c, acc, stg, bias_s, rpf, wg * 64 + (warp & 3) * 16, lane, ti);
+      epilogue<NI, RES, F16>(p, c, acc, stg, bias_s, rpf, wg * 64 + (warp & 3) * 16, lane, ti);
     }
   }
   if constexpr (RECORDS) ptx::tma_store_wait_all();  // the records' bulk stores complete before the CTA exits
@@ -877,27 +951,28 @@ int instr_n(int bn) { return bn <= 16 ? 16 : (bn + 31) / 32 * 32; }
 
 typedef void (*KernelFn)(ConvK);
 int ctas_for(int ni) { return ni <= 96 ? 2 : 1; }  // Occupancy<NI>::CTAS
-template <bool RES>
+template <bool RES, bool F16>
 KernelFn kernel_for(int ni) {
   switch (ni) {
-    case 16: return conv_wgmma_kernel<16, false, RES>;
-    case 32: return conv_wgmma_kernel<32, false, RES>;
-    case 64: return conv_wgmma_kernel<64, false, RES>;
-    case 96: return conv_wgmma_kernel<96, false, RES>;
-    case 128: return conv_wgmma_kernel<128, false, RES>;
-    case 160: return conv_wgmma_kernel<160, false, RES>;
-    case 192: return conv_wgmma_kernel<192, false, RES>;
-    case 224: return conv_wgmma_kernel<224, false, RES>;
-    case 256: return conv_wgmma_kernel<256, false, RES>;
+    case 16: return conv_wgmma_kernel<16, false, RES, F16>;
+    case 32: return conv_wgmma_kernel<32, false, RES, F16>;
+    case 64: return conv_wgmma_kernel<64, false, RES, F16>;
+    case 96: return conv_wgmma_kernel<96, false, RES, F16>;
+    case 128: return conv_wgmma_kernel<128, false, RES, F16>;
+    case 160: return conv_wgmma_kernel<160, false, RES, F16>;
+    case 192: return conv_wgmma_kernel<192, false, RES, F16>;
+    case 224: return conv_wgmma_kernel<224, false, RES, F16>;
+    case 256: return conv_wgmma_kernel<256, false, RES, F16>;
     default: return nullptr;
   }
 }
 // compact records need det_no > 180, so an N tile of at least 192 columns
+template <bool F16>
 KernelFn records_kernel_for(int ni) {
   switch (ni) {
-    case 192: return conv_wgmma_kernel<192, true>;
-    case 224: return conv_wgmma_kernel<224, true>;
-    case 256: return conv_wgmma_kernel<256, true>;
+    case 192: return conv_wgmma_kernel<192, true, false, F16>;
+    case 224: return conv_wgmma_kernel<224, true, false, F16>;
+    case 256: return conv_wgmma_kernel<256, true, false, F16>;
     default: return nullptr;
   }
 }
@@ -988,8 +1063,12 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
   const bool records = d->mode == MODE_DETECT && d->det_decode == 2 && d->det_no > 180 &&
                        ((d->det_no - 180 + 1) + 3) / 4 * 4 <= 64 && !(d->flags & Y5OBB_CONV_DETECT_GENERIC);
   const bool res_epi = d->mode == MODE_CONV && d->res;  // residual vectors loaded when each tile starts
-  o->fn = records ? records_kernel_for(ni) : (res_epi ? kernel_for<true>(ni) : kernel_for<false>(ni));
-  const int inst = records ? 1 : (res_epi ? 2 : 0);
+  const bool f16 = (d->flags & Y5OBB_CONV_F16) != 0;
+  if (f16)
+    o->fn = records ? records_kernel_for<true>(ni) : (res_epi ? kernel_for<true, true>(ni) : kernel_for<false, true>(ni));
+  else
+    o->fn = records ? records_kernel_for<false>(ni) : (res_epi ? kernel_for<true, false>(ni) : kernel_for<false, false>(ni));
+  const int inst = (records ? 1 : (res_epi ? 2 : 0)) + (f16 ? 3 : 0);
   if (!o->fn) {
     delete o;
     return Y5OBB_EINVAL;
@@ -1089,7 +1168,7 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     delete o;
     return Y5OBB_EINVAL;
   }
-  static bool attr_set[3][257] = {};  // per instantiation (NI; plain, records, residual)
+  static bool attr_set[6][257] = {};  // per instantiation (NI; plain, records, residual; bf16, then fp16)
   if (!attr_set[inst][ni]) {
     // all of the unified L1 / shared memory as shared memory, so that two 112 KB CTAs fit beside each other
     cudaError_t e = cudaFuncSetAttribute(o->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
@@ -1164,10 +1243,12 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     }
   } else {
     // rows of rw floats: 16-byte vector stores when rw % 4 == 0 (always for records), element stores otherwise
+    // (fp16 plans write fp16 rows, 8-byte vectors, unless they write records)
     const int rw = d->det_decode == 2 ? k.det_rec_w : d->det_no;
-    const uintptr_t align = rw % 4 ? 3 : 15;
+    const bool half_rows = f16 && d->det_decode != 2;
+    const uintptr_t align = half_rows ? (rw % 4 ? 1 : 7) : (rw % 4 ? 3 : 15);
     if (!d->det_out || (d->det_decode == 2 && d->det_no <= 180) ||
-        (reinterpret_cast<uintptr_t>(d->det_out + (size_t)d->det_row_off * rw) & align)) {
+        ((reinterpret_cast<uintptr_t>(d->det_out) + (size_t)d->det_row_off * rw * (half_rows ? 2 : 4)) & align)) {
       delete o;
       return Y5OBB_EINVAL;
     }
@@ -1191,7 +1272,7 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
       box[1] = (cuuint32_t)k.Wt;
       es[1] = 1;
     }
-    CUresult r = enc(&k.tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(d->in), dims, strides, box, es,
+    CUresult r = enc(&k.tmA, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(d->in), dims, strides, box, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
@@ -1205,7 +1286,7 @@ int y5obb_conv_create(const y5obb_conv_desc* d, y5obb_conv_t** out) {
     cuuint64_t strides[1] = {(cuuint64_t)cin_pad * 2};
     cuuint32_t box[2] = {(cuuint32_t)bk, (cuuint32_t)ni};
     cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(&k.tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(d->w), dims, strides, box, es,
+    CUresult r = enc(&k.tmB, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(d->w), dims, strides, box, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {

@@ -15,6 +15,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "stage.cuh"
 
 namespace y5obb {
 namespace {
@@ -78,8 +79,9 @@ __device__ __forceinline__ void lb_pixel(const Desc& d, const uint8_t* __restric
   }
 }
 
+template <typename E>
 __global__ void k_letterbox_s2d_u8(const uint8_t* __restrict__ src, const Desc* __restrict__ desc, int B, int Hp, int Wp,
-                                   __nv_bfloat16* __restrict__ out, int pad_cols) {
+                                   E* __restrict__ out, int pad_cols) {
   const int Ho = Hp >> 1, Wo = Wp >> 1;
   const int32_t* tab = reinterpret_cast<const int32_t*>(desc);
   const long long total = (long long)B * Ho * Wo;
@@ -94,15 +96,13 @@ __global__ void k_letterbox_s2d_u8(const uint8_t* __restrict__ src, const Desc* 
       const int y = 2 * ho + (q >> 1) - d.top, x = 2 * wo + (q & 1) - d.left;
       uint8_t px[3] = {114, 114, 114};
       if (y >= 0 && y < d.new_h && x >= 0 && x < d.new_w) lb_pixel(d, src + d.src_off, tab, y, x, px);
-      v[q * 3] = (float)px[2] / 255.0f;  // BGR -> RGB
-      v[q * 3 + 1] = (float)px[1] / 255.0f;
-      v[q * 3 + 2] = (float)px[0] / 255.0f;
+      v[q * 3] = u8_value(px[2], out);  // BGR -> RGB
+      v[q * 3 + 1] = u8_value(px[1], out);
+      v[q * 3 + 2] = u8_value(px[0], out);
     }
     v[12] = v[13] = v[14] = v[15] = 0.f;
     uint4 o[2];
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    pack16(v, out, o);
     uint4* dst = reinterpret_cast<uint4*>(out + ((r * (Wo + 2 * pad_cols)) + wo + pad_cols) * 16);
     dst[0] = o[0];
     dst[1] = o[1];
@@ -123,8 +123,9 @@ using namespace y5obb;
 
 extern "C" {
 
-int y5obb_letterbox_s2d_u8(const uint8_t* src, int64_t src_bytes, const void* desc_dev, const y5obb_letterbox_desc* desc_host,
-                           int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16, int pad_cols, void* stream) {
+static int letterbox_s2d_u8(bool f16, const uint8_t* src, int64_t src_bytes, const void* desc_dev,
+                            const y5obb_letterbox_desc* desc_host, int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16,
+                            int pad_cols, void* stream) {
   if (!src || !desc_dev || !desc_host || !out_nhwc16 || B <= 0 || Hp <= 0 || Wp <= 0 || (Hp & 1) || (Wp & 1) || pad_cols < 0 ||
       src_bytes <= 0 || desc_bytes < (int64_t)B * (int64_t)sizeof(y5obb_letterbox_desc) || (desc_bytes & 3))
     return Y5OBB_EINVAL;
@@ -165,10 +166,24 @@ int y5obb_letterbox_s2d_u8(const uint8_t* src, int64_t src_bytes, const void* de
   }
   const long long total = (long long)B * (Hp / 2) * (Wp / 2);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  k_letterbox_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(src, static_cast<const y5obb_letterbox_desc*>(desc_dev), B, Hp, Wp,
-                                                            static_cast<__nv_bfloat16*>(out_nhwc16), pad_cols);
+  const Desc* dd = static_cast<const y5obb_letterbox_desc*>(desc_dev);
+  if (f16)
+    k_letterbox_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(src, dd, B, Hp, Wp, static_cast<__half*>(out_nhwc16), pad_cols);
+  else
+    k_letterbox_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(src, dd, B, Hp, Wp, static_cast<__nv_bfloat16*>(out_nhwc16),
+                                                              pad_cols);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
+}
+
+int y5obb_letterbox_s2d_u8(const uint8_t* src, int64_t src_bytes, const void* desc_dev, const y5obb_letterbox_desc* desc_host,
+                           int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16, int pad_cols, void* stream) {
+  return letterbox_s2d_u8(false, src, src_bytes, desc_dev, desc_host, desc_bytes, B, Hp, Wp, out_nhwc16, pad_cols, stream);
+}
+
+int y5obb_letterbox_s2d_u8_f16(const uint8_t* src, int64_t src_bytes, const void* desc_dev, const y5obb_letterbox_desc* desc_host,
+                               int64_t desc_bytes, int B, int Hp, int Wp, void* out_nhwc16, int pad_cols, void* stream) {
+  return letterbox_s2d_u8(true, src, src_bytes, desc_dev, desc_host, desc_bytes, B, Hp, Wp, out_nhwc16, pad_cols, stream);
 }
 
 }  // extern "C"

@@ -22,6 +22,7 @@
 // duplicate cells (atomicAdd, order-dependent in the last bit).
 #include <cub/device/device_scan.cuh>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <algorithm>
 #include <cstring>
@@ -341,22 +342,37 @@ struct HeadK {
 // k_head_rows takes both blocks as its launch parameters (4 KB at most on sm_90)
 static_assert(sizeof(LossK) + sizeof(HeadK) <= 4096, "loss kernel parameters exceed the 4 KB launch-parameter limit");
 
-// 8 bf16 products of two 16-byte vectors, accumulated in order into acc
+// 8 bf16 (F16: fp16) products of two 16-byte vectors, accumulated in order into acc
+template <bool F16>
+__device__ __forceinline__ float2 to_float2(const uint32_t& v) {
+  if constexpr (F16) return __half22float2(*reinterpret_cast<const __half2*>(&v));
+  else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v));
+}
+template <bool F16>
 __device__ __forceinline__ float dot8(const uint4& x, const uint4& y, float acc) {
-  const __nv_bfloat162* a = reinterpret_cast<const __nv_bfloat162*>(&x);
-  const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&y);
+  const uint32_t* a = reinterpret_cast<const uint32_t*>(&x);
+  const uint32_t* b = reinterpret_cast<const uint32_t*>(&y);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float2 u = __bfloat1622float2(a[i]), v = __bfloat1622float2(b[i]);
+    const float2 u = to_float2<F16>(a[i]), v = to_float2<F16>(b[i]);
     acc = fmaf(u.x, v.x, acc);
     acc = fmaf(u.y, v.y, acc);
   }
   return acc;
 }
 
+// The logit the loss reads: bias + acc, and for an fp16 plan (F16: fp16 features and weights) that value rounded to fp16, the
+// half Detect conv's output that val.py:198-199 widens with `x.float()`
+template <bool F16>
+__device__ __forceinline__ float head_logit(float bias, float acc) {
+  if constexpr (F16) return __half2float(__float2half_rn(bias + acc));
+  else return bias + acc;
+}
+
 // obj logits of one level: head_obj[cell_off + ((b * na + a) * H + y) * W + x] = bias[a*no+4] + sum_c feat[b,y,x,c] w[a*no+4, c].
 // An N = na GEMM bound by the feature read: G lanes (a power of two dividing C/8) share a pixel, every feature byte is read once
 // with 16-byte loads, the na weight rows sit in shared memory.
+template <bool F16>
 __global__ void __launch_bounds__(256) k_head_obj(LossK L, HeadLevel h, int lvl, int G) {
   extern __shared__ uint4 s_w[];  // [na][C / 8]
   const int C8 = h.C / 8;
@@ -386,7 +402,7 @@ __global__ void __launch_bounds__(256) k_head_obj(LossK L, HeadLevel h, int lvl,
         const uint4 v = __ldg(reinterpret_cast<const uint4*>(f + c8 * 8));
 #pragma unroll
         for (int a = 0; a < 3; ++a)
-          if (a < L.na) acc[a] = dot8(v, s_w[a * C8 + c8], acc[a]);
+          if (a < L.na) acc[a] = dot8<F16>(v, s_w[a * C8 + c8], acc[a]);
       }
     }
     for (int o = G >> 1; o; o >>= 1) {
@@ -396,13 +412,14 @@ __global__ void __launch_bounds__(256) k_head_obj(LossK L, HeadLevel h, int lvl,
     if (valid && g == 0) {
 #pragma unroll
       for (int a = 0; a < 3; ++a)
-        if (a < L.na) out[(((long long)b * L.na + a) * H + y) * W + x] = h.bias[a * L.no + 4] + acc[a];
+        if (a < L.na) out[(((long long)b * L.na + a) * H + y) * W + x] = head_logit<F16>(h.bias[a * L.no + 4], acc[a]);
     }
   }
 }
 
 // the no logits of every matched row (after k_match and the scan): a gathered GEMV per row, one warp per candidate, written to
 // head_rows[rank * no + j] = bias[a*no+j] + sum_c feat[b,gj,gi,c] w[a*no+j, c]
+template <bool F16>
 __global__ void k_head_rows(LossK L, HeadK hk) {
   const int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -422,7 +439,7 @@ __global__ void k_head_rows(LossK L, HeadK hk) {
 #pragma unroll
       for (int k = 0; k < 4; ++k)
         if (j0 + k < L.no)
-          acc[k] = dot8(v, __ldg(reinterpret_cast<const uint4*>(w + (long long)(j0 + k) * h.C + c8 * 8)), acc[k]);
+          acc[k] = dot8<F16>(v, __ldg(reinterpret_cast<const uint4*>(w + (long long)(j0 + k) * h.C + c8 * 8)), acc[k]);
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) {
@@ -430,7 +447,7 @@ __global__ void k_head_rows(LossK L, HeadK hk) {
       for (int k = 0; k < 4; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
     }
     if (lane < 4 && j0 + lane < L.no)
-      out[j0 + lane] = bias[j0 + lane] + (lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]);
+      out[j0 + lane] = head_logit<F16>(bias[j0 + lane], lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3]);
   }
 }
 
@@ -622,8 +639,9 @@ int fill(LossK& L, const y5obb_loss_desc* d, void* ws, size_t ws_bytes, size_t* 
   return Y5OBB_OK;
 }
 
-// The forward shared by both logit sources; hk != nullptr computes the logits from the Detect inputs first.
-int forward(LossK& L, const HeadK* hk, float* loss1, float* items4, cudaStream_t st) {
+// The forward shared by both logit sources; hk != nullptr computes the logits from the Detect inputs first (f16: fp16
+// features and weights, logits rounded to fp16).
+int forward(LossK& L, const HeadK* hk, float* loss1, float* items4, cudaStream_t st, bool f16 = false) {
   if (L.nt > 0 && !L.targets) return Y5OBB_EINVAL;
   Y5_CUDA(cudaMemsetAsync(L.winner, 0xFF, (size_t)L.cell_off[L.nl] * sizeof(int), st));
   if (L.ncand > 0) {
@@ -632,7 +650,7 @@ int forward(LossK& L, const HeadK* hk, float* loss1, float* items4, cudaStream_t
     Y5_CUDA(cub::DeviceScan::ExclusiveSum(L.scan_tmp, L.scan_bytes, L.flag, L.rank, L.ncand, st));
     const long long threads = (long long)L.ncand * 32;
     if (hk) {
-      k_head_rows<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(L, *hk);
+      (f16 ? k_head_rows<true> : k_head_rows<false>)<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(L, *hk);
       Y5_LAUNCH_CHECK();
     }
     k_rows<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(L);
@@ -650,7 +668,7 @@ int forward(LossK& L, const HeadK* hk, float* loss1, float* items4, cudaStream_t
       while (G < 32 && C8 % (2 * G) == 0) G *= 2;
       const long long threads = (long long)L.B * L.H[lvl] * L.W[lvl] * G;
       const int grid = (int)std::min<long long>((threads + 255) / 256, (long long)sm_count() * 8);
-      k_head_obj<<<grid, 256, (size_t)L.na * C8 * sizeof(uint4), st>>>(L, h, lvl, G);
+      (f16 ? k_head_obj<true> : k_head_obj<false>)<<<grid, 256, (size_t)L.na * C8 * sizeof(uint4), st>>>(L, h, lvl, G);
       Y5_LAUNCH_CHECK();
     }
     k_obj<<<L.obj_blocks[lvl], OBJ_THREADS, 0, st>>>(L, lvl);
@@ -719,8 +737,8 @@ size_t y5obb_loss_head_workspace_bytes(const y5obb_loss_desc* d, const y5obb_los
   return need;
 }
 
-int y5obb_loss_forward_head(const y5obb_loss_desc* d, const y5obb_loss_head* head, float* loss1, float* items4,
-                            void* workspace, size_t workspace_bytes, void* stream) {
+static int loss_forward_head(bool f16, const y5obb_loss_desc* d, const y5obb_loss_head* head, float* loss1, float* items4,
+                             void* workspace, size_t workspace_bytes, void* stream) {
   if (!loss1 || !items4 || !workspace) return Y5OBB_EINVAL;
   y5obb_loss_desc dd;
   HeadK hk;
@@ -730,7 +748,17 @@ int y5obb_loss_forward_head(const y5obb_loss_desc* d, const y5obb_loss_head* hea
   size_t need = 0;
   rc = fill(L, &dd, workspace, workspace_bytes, &need, true);
   if (rc) return rc;
-  return forward(L, &hk, loss1, items4, (cudaStream_t)stream);
+  return forward(L, &hk, loss1, items4, (cudaStream_t)stream, f16);
+}
+
+int y5obb_loss_forward_head(const y5obb_loss_desc* d, const y5obb_loss_head* head, float* loss1, float* items4,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  return loss_forward_head(false, d, head, loss1, items4, workspace, workspace_bytes, stream);
+}
+
+int y5obb_loss_forward_head_f16(const y5obb_loss_desc* d, const y5obb_loss_head* head, float* loss1, float* items4,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  return loss_forward_head(true, d, head, loss1, items4, workspace, workspace_bytes, stream);
 }
 
 int y5obb_loss_backward(const y5obb_loss_desc* d, const float* grad_loss, void* workspace, size_t workspace_bytes,

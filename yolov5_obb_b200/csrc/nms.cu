@@ -16,6 +16,7 @@
 // Algorithmic bytes per box: 24 in (5 floats + score) + 8 out per kept box; the bit-matrix is
 // internal traffic (8 bytes per 64x64 tile row, upper triangle only).
 #include <cooperative_groups.h>
+#include <cuda_fp16.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -693,6 +694,15 @@ struct PPArgs {
   int compact;    // 1: rows are (cx, cy, w, h, obj, cls[nc], theta index) records written by the Detect epilogue
 };
 
+// conf = obj * cls: one fp32 rounding, then, for the records of an fp16 plan (HALF, Y5OBB_NMS_HALF), the rounding to fp16
+// of general.py:820's half `*=` (the product of two fp16 values is exact in fp32, so this is torch's single rounding)
+template <bool HALF>
+__device__ __forceinline__ float rec_conf(float cls, float obj) {
+  const float v = __fmul_rn(cls, obj);
+  if constexpr (HALF) return __half2float(__float2half_rn(v));
+  else return v;
+}
+
 __global__ void k_pp_count(PPArgs a, int* __restrict__ cnt) {
   const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -838,6 +848,7 @@ __global__ void k_pp_emit(PPArgs a, const int* __restrict__ cnt, const int* __re
 // ---- compact records (Y5OBB_NMS_COMPACT_PRED): one THREAD per anchor row.  A row is 96 B and almost every row fails the
 // objectness test on its first read, so a warp per row (the layout the 800-byte tensor rows want) would only schedule warps.
 // Same arithmetic, same candidate order (ascending class inside a row) as k_pp_count / k_pp_emit above.
+template <bool HALF>
 __global__ void k_pp_count_rec(PPArgs a, int* __restrict__ cnt) {
   const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= a.rows) return;
@@ -847,12 +858,12 @@ __global__ void k_pp_count_rec(PPArgs a, int* __restrict__ cnt) {
   if (obj > a.conf) {
     if (a.multi_label) {
       for (int j = 0; j < a.nc; ++j)
-        n += ((__fmul_rn(p[5 + j], obj) > a.conf) && ((a.class_mask >> (j & 63)) & 1ull)) ? 1 : 0;
+        n += ((rec_conf<HALF>(p[5 + j], obj) > a.conf) && ((a.class_mask >> (j & 63)) & 1ull)) ? 1 : 0;
     } else {
       float bv = -INFINITY;
       int bj = 0x7fffffff;
       for (int j = 0; j < a.nc; ++j) {
-        const float v = __fmul_rn(p[5 + j], obj);
+        const float v = rec_conf<HALF>(p[5 + j], obj);
         if (v > bv) {
           bv = v;
           bj = j;
@@ -864,6 +875,7 @@ __global__ void k_pp_count_rec(PPArgs a, int* __restrict__ cnt) {
   cnt[row] = n;
 }
 
+template <bool HALF>
 __global__ void k_pp_emit_rec(PPArgs a, const int* __restrict__ cnt, const int* __restrict__ off, long long capacity,
                               float* __restrict__ dets5, float* __restrict__ scores, int32_t* __restrict__ image_ids,
                               float* __restrict__ out7, int64_t* __restrict__ n_valid) {
@@ -908,14 +920,14 @@ __global__ void k_pp_emit_rec(PPArgs a, const int* __restrict__ cnt, const int* 
   };
   if (a.multi_label) {
     for (int j = 0; j < a.nc; ++j) {
-      const float sc = __fmul_rn(p[5 + j], obj);
+      const float sc = rec_conf<HALF>(p[5 + j], obj);
       if ((sc > a.conf) && ((a.class_mask >> (j & 63)) & 1ull)) put(j, sc);
     }
   } else {
     float cv = -INFINITY;
     int cj = 0x7fffffff;
     for (int j = 0; j < a.nc; ++j) {
-      const float v = __fmul_rn(p[5 + j], obj);
+      const float v = rec_conf<HALF>(p[5 + j], obj);
       if (v > cv) {
         cv = v;
         cj = j;
@@ -1164,7 +1176,7 @@ using namespace y5obb;
 
 extern "C" {
 
-int y5obb_abi_version(void) { return 1; }
+int y5obb_abi_version(void) { return 2; }
 int y5obb_last_cuda_error(void) { return g_last_cuda_error; }
 const char* y5obb_build_info(void) { return "liby5obb sm_90a " __DATE__ " " __TIME__; }
 
@@ -1218,6 +1230,8 @@ int y5obb_nms_obb_f32(const float* pred, int64_t batch, int64_t anchors, int no,
   if (w.total > workspace_bytes) return Y5OBB_EWORKSPACE;
   PPArgs a;
   a.compact = (flags & Y5OBB_NMS_COMPACT_PRED) ? 1 : 0;
+  const bool half = (flags & Y5OBB_NMS_HALF) != 0;
+  if (half && !a.compact) return Y5OBB_EINVAL;
   a.row_w = a.compact ? ((nc + 6) + 3) / 4 * 4 : no;
   a.pred = pred;
   a.rows = rows;
@@ -1235,13 +1249,13 @@ int y5obb_nms_obb_f32(const float* pred, int64_t batch, int64_t anchors, int no,
   if (split) Y5_CUDA(cudaMemsetAsync(w.far_flag, 0, sizeof(int), st));
   const unsigned g = (unsigned)((rows * 32 + 255) / 256);
   const unsigned g1 = (unsigned)((rows + 255) / 256);
-  if (a.compact) k_pp_count_rec<<<g1, 256, 0, st>>>(a, w.cnt);
+  if (a.compact) (half ? k_pp_count_rec<true> : k_pp_count_rec<false>)<<<g1, 256, 0, st>>>(a, w.cnt);
   else k_pp_count<<<g, 256, 0, st>>>(a, w.cnt);
   Y5_LAUNCH_CHECK();
   size_t sb = w.scan_bytes;
   Y5_CUDA(cub::DeviceScan::ExclusiveSum(w.scan_tmp, sb, w.cnt, w.off, (int)rows, st));
   if (a.compact)
-    k_pp_emit_rec<<<g1, 256, 0, st>>>(a, w.cnt, w.off, max_candidates, w.dets5, w.scores, w.image_ids, w.out7, w.n_valid);
+    (half ? k_pp_emit_rec<true> : k_pp_emit_rec<false>)<<<g1, 256, 0, st>>>(a, w.cnt, w.off, max_candidates, w.dets5, w.scores, w.image_ids, w.out7, w.n_valid);
   else
     k_pp_emit<<<g, 256, 0, st>>>(a, w.cnt, w.off, max_candidates, w.dets5, w.scores, w.image_ids, w.out7, w.n_valid);
   Y5_LAUNCH_CHECK();

@@ -19,15 +19,17 @@
 
 #include "common.cuh"
 #include "geom.cuh"
+#include "stage.cuh"
 
 namespace y5obb {
 namespace {
 
 using namespace geom;
 
+template <typename E>
 __global__ void k_scene_tiles_s2d_u8(const uint8_t* __restrict__ scene, long long H, long long W,
                                      const int32_t* __restrict__ origins, int T, int S, int size, int border,
-                                     __nv_bfloat16* __restrict__ out, int pad_cols) {
+                                     E* __restrict__ out, int pad_cols) {
   const int Ho = size >> 1, Wo = size >> 1;
   const long long total = (long long)T * Ho * Wo;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -53,13 +55,11 @@ __global__ void k_scene_tiles_s2d_u8(const uint8_t* __restrict__ scene, long lon
         }
       }
 #pragma unroll
-      for (int c = 0; c < 3; ++c) v[d * 3 + c] = (float)px[c] / 255.0f;
+      for (int c = 0; c < 3; ++c) v[d * 3 + c] = u8_value(px[c], out);
     }
     v[12] = v[13] = v[14] = v[15] = 0.f;
     uint4 o[2];
-    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) h[e] = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    pack16(v, out, o);
     uint4* dst = reinterpret_cast<uint4*>(out + ((r * (Wo + 2 * pad_cols)) + wo + pad_cols) * 16);
     dst[0] = o[0];
     dst[1] = o[1];
@@ -215,18 +215,32 @@ using namespace y5obb;
 
 extern "C" {
 
-int y5obb_scene_tiles_s2d_u8(const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles, int subsize,
-                             int size, int border, void* out_nhwc16, int pad_cols, void* stream) {
+static int scene_tiles_s2d_u8(bool f16, const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles,
+                              int subsize, int size, int border, void* out_nhwc16, int pad_cols, void* stream) {
   if (!scene_hwc || !origins2 || !out_nhwc16 || H <= 0 || W <= 0 || n_tiles <= 0 || subsize <= 0 || (size & 1) || size <= 0 ||
       border < 0 || border + subsize > size || pad_cols < 0)
     return Y5OBB_EINVAL;
   if (reinterpret_cast<uintptr_t>(out_nhwc16) & 15) return Y5OBB_EINVAL;
   const long long total = (long long)n_tiles * (size / 2) * (size / 2);
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  k_scene_tiles_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(scene_hwc, H, W, origins2, n_tiles, subsize, size, border,
-                                                              static_cast<__nv_bfloat16*>(out_nhwc16), pad_cols);
+  if (f16)
+    k_scene_tiles_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(scene_hwc, H, W, origins2, n_tiles, subsize, size, border,
+                                                                static_cast<__half*>(out_nhwc16), pad_cols);
+  else
+    k_scene_tiles_s2d_u8<<<grid, 256, 0, (cudaStream_t)stream>>>(scene_hwc, H, W, origins2, n_tiles, subsize, size, border,
+                                                                static_cast<__nv_bfloat16*>(out_nhwc16), pad_cols);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
+}
+
+int y5obb_scene_tiles_s2d_u8(const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles, int subsize,
+                             int size, int border, void* out_nhwc16, int pad_cols, void* stream) {
+  return scene_tiles_s2d_u8(false, scene_hwc, H, W, origins2, n_tiles, subsize, size, border, out_nhwc16, pad_cols, stream);
+}
+
+int y5obb_scene_tiles_s2d_u8_f16(const uint8_t* scene_hwc, int64_t H, int64_t W, const int32_t* origins2, int n_tiles,
+                                 int subsize, int size, int border, void* out_nhwc16, int pad_cols, void* stream) {
+  return scene_tiles_s2d_u8(true, scene_hwc, H, W, origins2, n_tiles, subsize, size, border, out_nhwc16, pad_cols, stream);
 }
 
 size_t y5obb_scene_merge_workspace_bytes(int64_t n_tiles, int max_det, int nc, const int64_t* class_cands_host) {

@@ -1,6 +1,6 @@
 """Inference plan: turns a yolo.Model into a fixed sequence of sm_90a kernel launches.
 
-Layout decisions (all NHWC bf16):
+Layout decisions (all NHWC bf16, or fp16 for a model whose parameters are fp16, see plan_dtype):
   * every tensor is a channel slice of some buffer; a producer whose output feeds a Concat
     (models/common.py:267-274) stores directly at its channel offset in the concat buffer;
   * nn.Upsample(2x nearest) is a second store of the producing conv's epilogue (out2x);
@@ -13,6 +13,8 @@ Layout decisions (all NHWC bf16):
   * Detect (models/yolo.py:49-81): one GEMM per level whose epilogue permutes, applies sigmoid and the
     grid/anchor decode and writes fp32 rows of the final [B, A, no] tensor.
 BatchNorm is folded into the conv weights exactly as utils/torch_utils.py:192-212 (fuse_conv_and_bn).
+fp16 plans are the reference's half inference (val.py --half, detect.py --half): the fused weights and biases are rounded to
+fp16, activations are fp16, and the Detect epilogue computes models/yolo.py:63-77 on a half tensor (Y5OBB_CONV_F16).
 """
 import ctypes
 import math
@@ -23,7 +25,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .conv import Conv as ConvOp, Slice, pack_weights, MODE_DETECT
+from .conv import Conv as ConvOp, Slice, pack_weights, MODE_DETECT, F16
 from .general import require_nc
 from .layout import _is, route, shapes, sources, stem_weight, stem_window
 from . import yolo as Y
@@ -45,15 +47,23 @@ def _conv_params(m):
     return fold_bn(m.conv, getattr(m, "bn", None))
 
 
+def plan_dtype(model) -> torch.dtype:
+    """The element type of a model's inference plans: fp16 when its parameters are fp16 (`model.half()`: a half model runs
+    half, as in torch), bf16 otherwise.  Plans of the two kinds are separate (yolo.Model keys them by it)."""
+    dts = {p.dtype for p in model.parameters()}
+    if torch.float16 in dts and len(dts) > 1:
+        raise RuntimeError(f"the model mixes parameter dtypes {sorted(str(d) for d in dts)}: call .half() or .float() on it")
+    return torch.float16 if dts == {torch.float16} else torch.bfloat16
+
+
 def stage_input(x: torch.Tensor, x_s2d: torch.Tensor) -> None:
     """The stem layout pass: x [B, 3, H, W] contiguous fp32 in [0, 1] or uint8 (the caller-side `/ 255` is folded in) ->
-    the space-to-depth stem input x_s2d, on the current stream."""
+    the space-to-depth stem input x_s2d (bf16, or fp16 for an fp16 plan), on the current stream."""
     B, _, H, W = x.shape
     L, st = _lib.lib(), _lib.stream_ptr(x_s2d.device)
-    if x.dtype == torch.uint8:
-        _lib.check(L.y5obb_stem_s2d_u8(x.data_ptr(), x_s2d.data_ptr(), B, H, W, 1, st), "y5obb_stem_s2d_u8")
-    else:
-        _lib.check(L.y5obb_stem_s2d(x.data_ptr(), x_s2d.data_ptr(), B, H, W, 1, st), "y5obb_stem_s2d")
+    sfx = "_f16" if x_s2d.dtype == torch.float16 else ""
+    name = ("y5obb_stem_s2d_u8" if x.dtype == torch.uint8 else "y5obb_stem_s2d") + sfx
+    _lib.check(getattr(L, name)(x.data_ptr(), x_s2d.data_ptr(), B, H, W, 1, st), name)
 
 
 class InferenceEngine:
@@ -65,8 +75,10 @@ class InferenceEngine:
                       `det_row_base` of every image on (default: an engine-owned tensor holding exactly this plan's rows);
         levels        the Detect levels to emit (default all).  Ops whose outputs reach no kept level are not emitted;
         descale       (inv_scale, flip_w): the Detect epilogue de-scales x y w h and de-flips x (y5obb_conv_desc.det_descale);
-        x_s2d         an external stem input [B, H/2, W/2 + 2, 16] bf16 whose two padding columns are zero (default: an
-                      engine-owned zeroed one).  Plans that share it read one staged image (EnsemblePlan)."""
+        x_s2d         an external stem input [B, H/2, W/2 + 2, 16] of the plan's dtype whose two padding columns are zero
+                      (default: an engine-owned zeroed one).  Plans that share it read one staged image (EnsemblePlan).
+        The plan's element type is plan_dtype(model): an fp16 plan's eval rows (`pred` without compact_detect) are fp16,
+        its compact records fp32 holding fp16 values."""
         device = torch.device(device)
         if device.type != "cuda":
             raise RuntimeError("InferenceEngine needs a CUDA device (sm_90a); there is no CPU path")
@@ -76,6 +88,10 @@ class InferenceEngine:
         if H % smax or W % smax:
             raise RuntimeError(f"image size {H}x{W} must be a multiple of the max stride {smax}")
         self.device, self.B, self.H, self.W = device, B, H, W
+        self.dtype = plan_dtype(model)
+        self.half = self.dtype == torch.float16
+        if self.half:
+            conv_flags |= F16
         self.ops = []          # (callable taking stream ptr)
         self._calls, self._graph = 0, None
         self._use_graph = os.environ.get("Y5OBB_NO_GRAPH", "0") != "1"
@@ -108,7 +124,7 @@ class InferenceEngine:
             n = B * h * w * c
             n_al = (n + 127) // 128 * 128   # 256-byte aligned starts (TMA wants 16)
             if arena["buf"] is None or arena["used"] + n_al > arena["buf"].numel():
-                arena["buf"] = torch.zeros(max(n_al, 128 << 20), dtype=torch.bfloat16, device=device)
+                arena["buf"] = torch.zeros(max(n_al, 128 << 20), dtype=self.dtype, device=device)
                 arena["used"] = 0
                 self.keep.append(arena["buf"])
             t = arena["buf"][arena["used"]:arena["used"] + n].view(B, h, w, c)
@@ -119,7 +135,10 @@ class InferenceEngine:
         self.out_slices = out   # per top-level layer: where its output lives (tests read them for teacher-forced parity)
 
         def add_conv(x, w, b, k, s, p, act, dst: Optional[Slice] = None, res=None, out2x=None, detd=None):
-            wp, bp = pack_weights(w.cpu(), b.cpu(), MODE_DETECT if detd else 0, detd["no"] if detd else 0)   # packed on the host
+            if self.half:   # model.half() rounds the fused bias too (attempt_load fuses in fp32 first); it stays an fp32 array
+                b = b.to(torch.float16).float()
+            wp, bp = pack_weights(w.cpu(), b.cpu(), MODE_DETECT if detd else 0, detd["no"] if detd else 0,
+                                  self.dtype)   # packed on the host
             if act and not detd:
                 bp = bp * 0.5   # the SiLU epilogue wants 0.5 * bias (Y5OBB_CONV_BIAS_HALVED)
             op = ConvOp(x, wp.to(device), bp.to(device), w.shape[0], k, s, p, act, out=dst, res=res, out2x=out2x, det=detd,
@@ -137,12 +156,12 @@ class InferenceEngine:
         # horizontal taps are then 48 CONTIGUOUS channels of an overlapping-window view (pixel stride 16)
         s2d_shape = (B, H // 2, W // 2 + 2, 16)
         if x_s2d is None:
-            self.x_s2d = torch.zeros(s2d_shape, dtype=torch.bfloat16, device=device)
+            self.x_s2d = torch.zeros(s2d_shape, dtype=self.dtype, device=device)
         else:
             _lib.require_cuda(x_s2d, "x_s2d")
-            if (tuple(x_s2d.shape) != s2d_shape or x_s2d.dtype != torch.bfloat16 or not x_s2d.is_contiguous()
+            if (tuple(x_s2d.shape) != s2d_shape or x_s2d.dtype != self.dtype or not x_s2d.is_contiguous()
                     or x_s2d.device != device):
-                raise RuntimeError(f"x_s2d must be a contiguous bf16 {list(s2d_shape)} tensor on {device}, got "
+                raise RuntimeError(f"x_s2d must be a contiguous {self.dtype} {list(s2d_shape)} tensor on {device}, got "
                                    f"{tuple(x_s2d.shape)} {x_s2d.dtype} on {x_s2d.device}")
             self.x_s2d = x_s2d
         self.keep.append(self.x_s2d)
@@ -197,7 +216,8 @@ class InferenceEngine:
                 add_conv(x, w1, b1, 1, 1, 0, True, Slice(cat4, 0, c_))
                 hh, ww = hw[i]
                 ptr, ps = cat4.data_ptr(), cat4.shape[3]
-                self.ops.append(lambda st, ptr=ptr, ps=ps, hh=hh, ww=ww, c_=c_: L.y5obb_sppf_pool(ptr, ps, B, hh, ww, c_, st))
+                pool = L.y5obb_sppf_pool_f16 if self.half else L.y5obb_sppf_pool
+                self.ops.append(lambda st, ptr=ptr, ps=ps, hh=hh, ww=ww, c_=c_: pool(ptr, ps, B, hh, ww, c_, st))
                 self.op_layers.append(i)
                 self.hbm_bytes += 2.0 * B * hh * ww * c_ * 4
                 w2, b2 = _conv_params(m.cv2)
@@ -214,16 +234,18 @@ class InferenceEngine:
         self.rec_w = ((det.nc + 6) + 3) // 4 * 4
         self.nc = det.nc
         width = self.rec_w if compact_detect else det.no
+        self.pred_dtype = torch.float16 if self.half and not compact_detect else torch.float32
         if det_out is None:
             if det_row_base:
                 raise RuntimeError("det_row_base needs an external det_out")
-            self.pred = torch.empty((B, self.rows_total, width), dtype=torch.float32, device=device)
+            self.pred = torch.empty((B, self.rows_total, width), dtype=self.pred_dtype, device=device)
         else:
             _lib.require_cuda(det_out, "det_out")
-            if (det_out.dtype != torch.float32 or not det_out.is_contiguous() or det_out.dim() != 3 or det_out.shape[0] != B
+            if (det_out.dtype != self.pred_dtype or not det_out.is_contiguous() or det_out.dim() != 3 or det_out.shape[0] != B
                     or det_out.shape[2] != width or det_out.device != device or det_row_base < 0
                     or det_row_base + self.rows_total > det_out.shape[1]):
-                raise RuntimeError(f"det_out must be a contiguous fp32 [{B}, >= {det_row_base + self.rows_total}, {width}] "
+                raise RuntimeError(f"det_out must be a contiguous {self.pred_dtype} [{B}, >= {det_row_base + self.rows_total}, "
+                                   f"{width}] "
                                    f"tensor on {device}, got {tuple(det_out.shape)} {det_out.dtype}")
             self.pred = det_out
         row_off = int(det_row_base)
@@ -242,20 +264,22 @@ class InferenceEngine:
                      detd=dict(out=self.pred, rows_per_image=self.pred.shape[1], row_off=row_off, no=det.no,
                                decode=2 if compact_detect else True,
                                stride=stride, anchors_px=anchors_px, descale=descale))
-            # the GEMM's operands: pack_weights rounds the same fp32 values to bf16, the bias stays fp32
-            self._head.append((out[f], w.reshape(w.shape[0], -1).to(torch.bfloat16).to(device), b.to(device)))
+            # the GEMM's operands: pack_weights rounds the same fp32 values to the plan's dtype, the bias stays fp32
+            self._head.append((out[f], w.reshape(w.shape[0], -1).to(self.dtype).to(device), b.to(device)))
             row_off += det.na * hw[f][0] * hw[f][1]
-        self.hbm_bytes += 4.0 * B * self.rows_total * det.no + 4.0 * B * 3 * H * W + 2.0 * self.x_s2d.numel()
+        self.hbm_bytes += (self.pred.element_size() * B * self.rows_total * det.no + 4.0 * B * 3 * H * W
+                           + 2.0 * self.x_s2d.numel())
         self.n_launches = len(self.ops) + 1
 
     def head_inputs(self):
-        """Per emitted Detect level: (input Slice, bf16 weight [na * no, C], fp32 bias [na * no]) - the Detect GEMM's operands.
+        """Per emitted Detect level: (input Slice, weight [na * no, C] of the plan's dtype, fp32 bias [na * no]) - the Detect
+        GEMM's operands.
         The input holds the features of the last forward until the next one, as `pred` does."""
         return list(self._head)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        """x: [B,3,H,W] fp32 in [0,1] (or uint8 0..255) on this engine's device -> pred [B, A, no] fp32
-        (engine-owned buffer, overwritten by the next call)."""
+        """x: [B,3,H,W] fp32 in [0,1] (or uint8 0..255) on this engine's device -> pred [B, A, no] fp32, fp16 for an fp16
+        plan (engine-owned buffer, overwritten by the next call).  A half image is widened exactly and rounded back."""
         _lib.require_cuda(x, "x")
         if tuple(x.shape) != (self.B, 3, self.H, self.W):
             raise RuntimeError(f"engine was planned for {(self.B, 3, self.H, self.W)}, got {tuple(x.shape)}")
@@ -351,11 +375,13 @@ class TTAPlan:
         self.nc, self.no = det.nc, det.no
         self.rec_w = ((det.nc + 6) + 3) // 4 * 4
         self.compact_detect = bool(compact_detect)
+        self.dtype = plan_dtype(model)
+        self.half = self.dtype == torch.float16
         if det_out is None:
             if det_row_base:
                 raise RuntimeError("det_row_base needs an external det_out")
-            det_out = torch.empty((B, self.rows_total, self.rec_w if compact_detect else det.no), dtype=torch.float32,
-                                  device=device)
+            det_out = torch.empty((B, self.rows_total, self.rec_w if compact_detect else det.no),
+                                  dtype=torch.float16 if self.half and not compact_detect else torch.float32, device=device)
         self.pred = det_out
         stems = [None] * len(self.branches) if stems is None else list(stems)
         if len(stems) != len(self.branches):
@@ -374,7 +400,8 @@ class TTAPlan:
     def resample(self, x: torch.Tensor, k: int) -> None:
         """scale_img of branch k (k >= 1) into that engine's x_s2d."""
         g, e = self.branches[k], self.engines[k]
-        fn = _lib.lib().y5obb_scale_img_s2d_u8 if x.dtype == torch.uint8 else _lib.lib().y5obb_scale_img_s2d
+        name = ("y5obb_scale_img_s2d_u8" if x.dtype == torch.uint8 else "y5obb_scale_img_s2d") + ("_f16" if self.half else "")
+        fn = getattr(_lib.lib(), name)
         _lib.check(fn(x.data_ptr(), e.x_s2d.data_ptr(), self.B, self.H, self.W, g["h"], g["w"], g["Hp"], g["Wp"],
                       1 if g["flip"] == 3 else 0, TTA_PAD, 1, _lib.stream_ptr(self.device)), "y5obb_scale_img_s2d")
 
@@ -437,15 +464,20 @@ class EnsemblePlan:
         if len(ncs) != 1:
             raise RuntimeError(f"ensemble members have different class counts {ncs}: their rows cannot be concatenated")
         require_nc(ncs[0], "EnsemblePlan")
+        dts = {plan_dtype(m) for m in models}
+        if len(dts) != 1:
+            raise RuntimeError("ensemble members mix fp16 and fp32 parameters: call .half() or .float() on the ensemble")
+        self.dtype = dts.pop()
+        self.half = self.dtype == torch.float16
         self.row_bases, self.rows_total = ensemble_layout(models, H, W, augment)
         self.device, self.B, self.H, self.W = device, B, H, W
         self.nc = ncs[0]
         self.no = self.nc + 185
         self.rec_w = ((self.nc + 6) + 3) // 4 * 4
         self.compact_detect, self.augment = bool(compact_detect), bool(augment)
-        self.pred = torch.empty((B, self.rows_total, self.rec_w if compact_detect else self.no), dtype=torch.float32,
-                                device=device)
-        self.x_s2d = torch.zeros((B, H // 2, W // 2 + 2, 16), dtype=torch.bfloat16, device=device)
+        self.pred = torch.empty((B, self.rows_total, self.rec_w if compact_detect else self.no),
+                                dtype=torch.float16 if self.half and not compact_detect else torch.float32, device=device)
+        self.x_s2d = torch.zeros((B, H // 2, W // 2 + 2, 16), dtype=self.dtype, device=device)
         self.steps = [(("stem",), lambda x: stage_input(x, self.x_s2d))]
         if not augment:
             self.members = [InferenceEngine(m, B, H, W, device, conv_flags, compact_detect, det_out=self.pred,
@@ -457,7 +489,7 @@ class EnsemblePlan:
             gss = [int(max(m.stride)) for m in models]
             stems = {}   # gs -> per branch stem input; branch 0 (scale 1, no padding) is the staged image itself
             for gs in sorted(set(gss)):
-                stems[gs] = [self.x_s2d] + [torch.zeros((B, g["Hp"] // 2, g["Wp"] // 2 + 2, 16), dtype=torch.bfloat16,
+                stems[gs] = [self.x_s2d] + [torch.zeros((B, g["Hp"] // 2, g["Wp"] // 2 + 2, 16), dtype=self.dtype,
                                                         device=device) for g in tta_geometry(H, W, gs)[0][1:]]
             self.members = [TTAPlan(m, B, H, W, device, compact_detect, conv_flags, det_out=self.pred, det_row_base=base,
                                     stems=stems[gs]) for m, base, gs in zip(models, self.row_bases, gss)]

@@ -52,6 +52,10 @@ class Ensemble(nn.ModuleList):
         """Drop every plan; the next call re-plans."""
         self._plans.clear()
 
+    def _precision_key(self):
+        """() for the bf16 plans, ("f16",) for the fp16 plans of a half ensemble (engine.plan_dtype)."""
+        return self[0]._precision_key()
+
     def _signature(self):
         return tuple(m._weights_signature() for m in self)
 
@@ -60,7 +64,7 @@ class Ensemble(nn.ModuleList):
             raise RuntimeError("an ensemble is an inference entry point: its members must be in eval mode")
         from .engine import EnsemblePlan
         device = torch.device(device)
-        key = (kind, tuple(shape), device.index) + ((int(slot),) if slot else ())
+        key = (kind, tuple(shape), device.index) + ((int(slot),) if slot else ()) + self._precision_key()
         plan = self._plans.get(key)
         sig = self._signature()
         if plan is None or plan._weights_sig != sig:
@@ -96,7 +100,7 @@ class Ensemble(nn.ModuleList):
             plan = self.tta_plan(tuple(x.shape), x.device, compact_detect=True, slot=slot)
         else:
             plan = self.records_plan(tuple(x.shape), x.device, slot)
-        return DetectRecords(plan.forward(x), plan.nc)
+        return DetectRecords(plan.forward(x), plan.nc, plan.half)
 
 
 def attempt_load(models):

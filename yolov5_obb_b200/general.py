@@ -4,6 +4,7 @@ replaced by one device pipeline (csrc/nms.cu: k_pp_* + batched rotated NMS) and 
 per-image counts at the end."""
 from typing import List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -23,10 +24,18 @@ def require_nc(nc: int, what: str) -> None:
 class DetectRecords:
     """What yolo.Model.detect_records returns: `data` [B, A, rec_w] fp32 rows (cx, cy, w, h, obj, cls[nc], theta index, pad)
     written by the Detect epilogue (engine-owned buffer, overwritten by the next forward), and the class count.  The theta index
-    is the first maximum of the row's 180 theta logits, i.e. what torch.max returns on their sigmoids (utils/general.py:822)."""
+    is the first maximum of the row's 180 theta logits, i.e. what torch.max returns on their sigmoids (utils/general.py:822).
+    half: the records of an fp16 plan - fp16 values, the theta index the first maximum of the fp16 sigmoids - which
+    non_max_suppression_obb post-processes with the reference's half arithmetic."""
 
-    def __init__(self, data: torch.Tensor, nc: int):
-        self.data, self.nc = data, int(nc)
+    def __init__(self, data: torch.Tensor, nc: int, half: bool = False):
+        self.data, self.nc, self.half = data, int(nc), bool(half)
+
+
+def half_threshold(conf_thres: float) -> float:
+    """conf_thres as `half_tensor > conf_thres` compares with it on the GPU: ATen casts the Python float to the tensor's
+    dtype (fp32 first, then fp16, as c10::Half's constructor from a double does)."""
+    return float(np.float16(np.float32(conf_thres)))
 
 
 def non_max_suppression_obb(prediction: torch.Tensor, conf_thres: float = 0.25, iou_thres: float = 0.45,
@@ -40,6 +49,7 @@ def non_max_suppression_obb(prediction: torch.Tensor, conf_thres: float = 0.25, 
         list of detections, len=batch_size, on (n,7) tensor per image [xylsθ, conf, cls] θ ∈ [-pi/2, pi/2)
     """
     compact = isinstance(prediction, DetectRecords)
+    half = compact and prediction.half
     if compact:
         nc_rec = prediction.nc
         prediction = prediction.data
@@ -68,7 +78,9 @@ def non_max_suppression_obb(prediction: torch.Tensor, conf_thres: float = 0.25, 
     # optimistic capacity (every kernel of the pipeline runs over `cap` slots); grown on overflow below
     cap = min(worst, max(B * 8192, 1 << 16, int(_CAP_HINT.get((B, A, nc), 0))))
     nosplit = _NO_SPLIT.get((B, A, nc), False)
-    args = (pred, B, A, no, nc, conf_thres, iou_thres, mask, agnostic, multi_label, max_det, nosplit, compact)
+    if half:   # general.py:797 and :830 compare half tensors with conf_thres
+        conf_thres = half_threshold(conf_thres)
+    args = (pred, B, A, no, nc, conf_thres, iou_thres, mask, agnostic, multi_label, max_det, nosplit, compact, half)
     if return_packed == "async":
         # no host read at all: (device [B, max_det, 7], device int64 [B + 1] = rows per image + total candidates, cap).
         # The caller checks counts[B] <= cap when it reads the counts (pipeline.DetectPipeline does, and re-runs).
@@ -82,7 +94,7 @@ def non_max_suppression_obb(prediction: torch.Tensor, conf_thres: float = 0.25, 
         c = counts.tolist()  # the one host read: rows per image (+ total candidates)
         if c[B] == -2:  # a box reaches another class's offset copy: the class-split shortcut is not exact here
             _NO_SPLIT[(B, A, nc)] = True
-            args = args[:-2] + (True, args[-1])
+            args = args[:-3] + (True,) + args[-2:]
             continue
         if c[B] <= cap:
             break
@@ -127,7 +139,7 @@ def _launch_graphed(args, cap):
 
 
 def _launch(args, cap, keep_ws=False):
-    pred, B, A, no, nc, conf_thres, iou_thres, mask, agnostic, multi_label, max_det, nosplit, compact = args
+    pred, B, A, no, nc, conf_thres, iou_thres, mask, agnostic, multi_label, max_det, nosplit, compact, half = args
     L = _lib.lib()
     dev = pred.device
     out = torch.empty((B, max_det, 7), dtype=torch.float32, device=dev)
@@ -140,7 +152,8 @@ def _launch(args, cap, keep_ws=False):
             _lib.workspace(nbytes, dev, f"nms_obb:{_lib.stream_ptr(dev)}")
         rc = L.y5obb_nms_obb_f32(pred.data_ptr(), B, A, no, nc, float(conf_thres), float(iou_thres), mask,
                                  int(bool(agnostic)), int(bool(multi_label)), int(max_det), MAX_NMS, float(MAX_WH),
-                                 _lib.NMS_STRICT_GT | (_lib.NMS_NO_CLASS_SPLIT if nosplit else 0) | (_lib.NMS_COMPACT_PRED if compact else 0),
+                                 _lib.NMS_STRICT_GT | (_lib.NMS_NO_CLASS_SPLIT if nosplit else 0) | (_lib.NMS_COMPACT_PRED if compact else 0)
+                                 | (_lib.NMS_HALF if half else 0),
                                  cap, out.data_ptr(),
                                  counts.data_ptr(), ws.data_ptr(),
                                  ws.numel(), _lib.stream_ptr(dev))

@@ -301,19 +301,20 @@ def pack_batch(images: Sequence[np.ndarray], placements: Sequence[Placement], Hp
 
 
 def letterbox_s2d(dev_buf: torch.Tensor, batch: PackedBatch, x_s2d: torch.Tensor, pad_cols: int = 1) -> None:
-    """Launches y5obb_letterbox_s2d_u8 on the current stream: dev_buf holds batch.host[:batch.nbytes] on the device,
-    x_s2d [B, Hp/2, Wp/2 + 2*pad_cols, 16] bf16 is the plan's stem input."""
+    """Launches y5obb_letterbox_s2d_u8 (_f16) on the current stream: dev_buf holds batch.host[:batch.nbytes] on the device,
+    x_s2d [B, Hp/2, Wp/2 + 2*pad_cols, 16] bf16 (fp16) is the plan's stem input."""
     _lib.require_cuda(dev_buf, "dev_buf")
     want = (batch.B, batch.Hp // 2, batch.Wp // 2 + 2 * pad_cols, 16)
-    if x_s2d.dtype != torch.bfloat16 or tuple(x_s2d.shape) != want or not x_s2d.is_contiguous():
-        raise RuntimeError(f"x_s2d must be contiguous bf16 {want}, got {x_s2d.dtype} {tuple(x_s2d.shape)}")
+    if x_s2d.dtype not in (torch.bfloat16, torch.float16) or tuple(x_s2d.shape) != want or not x_s2d.is_contiguous():
+        raise RuntimeError(f"x_s2d must be contiguous bf16 or fp16 {want}, got {x_s2d.dtype} {tuple(x_s2d.shape)}")
+    name = "y5obb_letterbox_s2d_u8" + ("_f16" if x_s2d.dtype == torch.float16 else "")
     if dev_buf.dtype != torch.uint8 or dev_buf.numel() < batch.nbytes:
         raise RuntimeError("dev_buf is smaller than the packed batch")
     base = dev_buf.data_ptr()
     with torch.cuda.device(dev_buf.device):
-        _lib.check(_lib.lib().y5obb_letterbox_s2d_u8(base + batch.src_off, batch.src_bytes, base, batch.host.data_ptr(),
-                                                     batch.desc_bytes, batch.B, batch.Hp, batch.Wp, x_s2d.data_ptr(), pad_cols,
-                                                     _lib.stream_ptr(dev_buf.device)), "y5obb_letterbox_s2d_u8")
+        _lib.check(getattr(_lib.lib(), name)(base + batch.src_off, batch.src_bytes, base, batch.host.data_ptr(),
+                                             batch.desc_bytes, batch.B, batch.Hp, batch.Wp, x_s2d.data_ptr(), pad_cols,
+                                             _lib.stream_ptr(dev_buf.device)), name)
 
 
 def scale_polys_batched(rows: torch.Tensor, counts: torch.Tensor, pad_gain: torch.Tensor) -> torch.Tensor:

@@ -158,7 +158,8 @@ class ComputeLoss:
     def head_items(self, engine, targets):
         """val.py:198-199's `compute_loss([x.float() for x in train_out], targets)[1]` for the eval forward an
         engine.InferenceEngine (Model.records_plan) has just run, without its raw head output: the loss reads logits computed
-        from the Detect inputs the plan keeps (y5obb_loss_forward_head).  targets: CUDA [nt, 187 | 8 | 7] as in __call__.
+        from the Detect inputs the plan keeps (y5obb_loss_forward_head; for an fp16 plan y5obb_loss_forward_head_f16, whose
+        logits are rounded to fp16 as the half Detect conv's are).  targets: CUDA [nt, 187 | 8 | 7] as in __call__.
         Returns device (loss [1], items [4]) = (lbox, lobj, lcls, ltheta); asynchronous, no autograd.  The features must still
         be those of the batch the targets belong to: call it before the plan's next forward."""
         from .engine import InferenceEngine
@@ -191,8 +192,9 @@ class ComputeLoss:
                 raise RuntimeError("y5obb_loss_head_workspace_bytes: invalid loss description or Detect inputs")
             st = _lib.stream_ptr(dev)
             ws = _lib.workspace(nbytes, dev, f"loss_head:{st}")
-            _lib.check(L.y5obb_loss_forward_head(ctypes.byref(d), ctypes.byref(h), loss.data_ptr(), items.data_ptr(),
-                                                 ws.data_ptr(), ws.numel(), st), "y5obb_loss_forward_head")
+            name = "y5obb_loss_forward_head_f16" if engine.half else "y5obb_loss_forward_head"
+            _lib.check(getattr(L, name)(ctypes.byref(d), ctypes.byref(h), loss.data_ptr(), items.data_ptr(),
+                                        ws.data_ptr(), ws.numel(), st), name)
         return loss, items
 
 

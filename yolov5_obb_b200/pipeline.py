@@ -275,7 +275,7 @@ class DetectPipeline:
         eng = self.model.records_plan((batch.B, 3, batch.Hp, batch.Wp), self.device, slot)
         lb.letterbox_s2d(buf, batch, eng.x_s2d, 1)
         pad_gain = buf[batch.pad_gain_off:batch.pad_gain_off + 12 * batch.B].view(torch.float32)
-        return DetectRecords(eng.forward_s2d(), eng.nc), pad_gain
+        return DetectRecords(eng.forward_s2d(), eng.nc, eng.half), pad_gain
 
     def _run_raw(self, raw_batches):
         """The loop of __call__ for packed raw batches: yields (input indices, [ImageDetections]) per batch, in batch order."""

@@ -187,11 +187,11 @@ class SceneDetector:
         n = min(B, T - t0)
         dev = scene.device
         eng = self.model.records_plan((B, 3, self.size, self.size), dev)
-        L = _lib.lib()
-        _lib.check(L.y5obb_scene_tiles_s2d_u8(scene.data_ptr(), scene.shape[0], scene.shape[1], org[t0].data_ptr(), n,
-                                              self.subsize, self.size, self.border, eng.x_s2d.data_ptr(), 1,
-                                              _lib.stream_ptr(dev)), "y5obb_scene_tiles_s2d_u8")
-        rec = DetectRecords(eng.forward_s2d(), eng.nc)
+        name = "y5obb_scene_tiles_s2d_u8" + ("_f16" if eng.half else "")
+        _lib.check(getattr(_lib.lib(), name)(scene.data_ptr(), scene.shape[0], scene.shape[1], org[t0].data_ptr(), n,
+                                             self.subsize, self.size, self.border, eng.x_s2d.data_ptr(), 1,
+                                             _lib.stream_ptr(dev)), name)
+        rec = DetectRecords(eng.forward_s2d(), eng.nc, eng.half)
         self.nc = eng.nc
         kw = dict(multi_label=True, max_det=self.max_det)
         if status is None:

@@ -290,7 +290,7 @@ class Validator:
         shape = (batch.B, 3, batch.Hp, batch.Wp)
         eng = self.model.records_plan(shape, self.device)
         lb.letterbox_s2d(buf, batch, eng.x_s2d, 1)
-        return DetectRecords(eng.forward_s2d(), eng.nc), shape
+        return DetectRecords(eng.forward_s2d(), eng.nc, eng.half), shape
 
     def __call__(self, batches) -> ValMetrics:
         nc = self.model.nc if hasattr(self.model, "nc") else self.model.model[-1].nc   # (an Ensemble has `nc`)

@@ -313,7 +313,7 @@ class Model(nn.Module):
         if self.training:
             return self.forward_train(x)
         from .engine import InferenceEngine
-        key = (tuple(x.shape), x.device.index)
+        key = (tuple(x.shape), x.device.index) + self._precision_key()
         eng = self._engines.get(key)
         # The inference plan folds BatchNorm into packed bf16 weights when it is built.  Parameters and statistics that
         # were updated in place since then (optimizer / EMA steps, load_state_dict, a training forward) show up in the
@@ -331,6 +331,9 @@ class Model(nn.Module):
         With a reserved arena (reserve_train_arena) the returned tensors live in it: the next training forward of ANY
         shape overwrites them."""
         from .train_engine import TrainEngine
+        if self._precision_key():
+            raise RuntimeError("training a model with fp16 parameters is not supported: fp16 plans are inference only "
+                               "(val.py / detect.py --half); train the fp32 model and call .half() on a copy for inference")
         in_hw = (int(x.shape[2]), int(x.shape[3]))
         hw = in_hw if size is None else (int(size[0]), int(size[1]))
         key = ("train", tuple(x.shape), x.device.index) + ((hw,) if hw != in_hw else ())
@@ -407,7 +410,7 @@ class Model(nn.Module):
             raise RuntimeError("test-time augmentation is an inference entry point (model.eval())")
         from .engine import TTAPlan
         device = torch.device(device)
-        key = ("tta", tuple(shape), device.index, bool(compact_detect)) + ((int(slot),) if slot else ())
+        key = ("tta", tuple(shape), device.index, bool(compact_detect)) + ((int(slot),) if slot else ()) + self._precision_key()
         plan = self._engines.get(key)
         sig = self._weights_signature()
         if plan is None or plan._weights_sig != sig:
@@ -428,9 +431,9 @@ class Model(nn.Module):
         from .general import DetectRecords
         if augment:
             plan = self.tta_plan(tuple(x.shape), x.device, compact_detect=True, slot=slot)
-            return DetectRecords(plan.forward(x), plan.nc)
+            return DetectRecords(plan.forward(x), plan.nc, plan.half)
         eng = self.records_plan(tuple(x.shape), x.device, slot)
-        return DetectRecords(eng.forward(x), eng.nc)
+        return DetectRecords(eng.forward(x), eng.nc, eng.half)
 
     def records_plan(self, shape, device, slot: int = 0):
         """The InferenceEngine behind detect_records for inputs of `shape` [B, 3, H, W] on `device`, re-planned when the weights
@@ -439,13 +442,19 @@ class Model(nn.Module):
             raise RuntimeError("detect_records is an inference entry point (model.eval())")
         from .engine import InferenceEngine
         device = torch.device(device)
-        key = ("records", tuple(shape), device.index) + ((int(slot),) if slot else ())
+        key = ("records", tuple(shape), device.index) + ((int(slot),) if slot else ()) + self._precision_key()
         eng = self._engines.get(key)
         sig = self._weights_signature()
         if eng is None or eng._weights_sig != sig:
             eng = self._engines[key] = InferenceEngine(self, shape[0], shape[2], shape[3], device, compact_detect=True)
             eng._weights_sig = sig
         return eng
+
+    def _precision_key(self):
+        """() for the bf16 plans, ("f16",) for the fp16 plans of a model whose parameters are fp16 (engine.plan_dtype): one
+        process can hold plans of both kinds."""
+        p = next(self.parameters(), None)   # (cheap: called per forward; engine.plan_dtype refuses mixed dtypes)
+        return ("f16",) if p is not None and p.dtype == torch.float16 else ()
 
     def _weights_signature(self):
         tr = getattr(self, "_sig_tensors", None)
