@@ -403,9 +403,12 @@ int y5obb_pack_plan_run(const y5obb_pack_plan_t* plan, void* stream);
 void y5obb_pack_plan_destroy(y5obb_pack_plan_t* plan);
 
 /* ---- fused SGD-Nesterov + EMA step -------------------------------------------------------------------------------
- * train.py:148-162,336-342 + utils/torch_utils.py:304-314 over every tensor in one launch.  group 0/1/2 index the per-step
- * learning-rate table (BatchNorm weights / decayed weights / biases); group -1 = EMA only (floating-point buffers);
- * ema may be NULL. */
+ * train.py:148-162,336-342 + utils/torch_utils.py:304-314 over every tensor in one launch, each op rounded as torch's
+ * foreach SGD and ModelEMA's per-tensor ops round it.  group 0/1/2 index the per-step learning-rate table (BatchNorm
+ * weights / decayed weights / biases); group -1 = EMA only (floating-point buffers), which needs an ema; a trainable
+ * entry's ema may be NULL.
+ * run: lr3 must not be NULL, momentum must be >= 0 and ema_decay (the double ModelEMA computes) must lie in [0, 1]; the
+ * EMA reads d and 1 - d (formed in double) as floats.  first_step != 0: the momentum buffers start as the gradient. */
 typedef struct y5obb_sgd_plan y5obb_sgd_plan_t;
 typedef struct {
   float* p;          /* parameter (fp32 master weight), updated in place */
@@ -417,7 +420,7 @@ typedef struct {
   int group;
 } y5obb_sgd_entry;
 int y5obb_sgd_ema_plan_create(const y5obb_sgd_entry* entries, int n, y5obb_sgd_plan_t** out);
-int y5obb_sgd_ema_plan_run(const y5obb_sgd_plan_t* plan, const float* lr3, float momentum, float ema_decay, int first_step,
+int y5obb_sgd_ema_plan_run(const y5obb_sgd_plan_t* plan, const float* lr3, float momentum, double ema_decay, int first_step,
                            void* stream);
 void y5obb_sgd_ema_plan_destroy(y5obb_sgd_plan_t* plan);
 
@@ -427,7 +430,8 @@ void y5obb_sgd_ema_plan_destroy(y5obb_sgd_plan_t* plan);
  * 0/1/2 index the per-step step-size table; group -1 = EMA only (floating-point buffers); ema may be NULL.
  * run: step_size3[k] = -lr_k / (1 - beta1^t) and bc2_sqrt = (1 - beta2^t)^0.5, computed in double and rounded to float as
  * torch does; beta1 / beta2 are the doubles of the parameter group (1 - beta1, beta2 and 1 - beta2 are formed in double
- * and rounded to float here, as torch's scalar arguments are).  beta1 and beta2 must lie in [0, 1), bc2_sqrt be > 0. */
+ * and rounded to float here, as torch's scalar arguments are).  beta1 and beta2 must lie in [0, 1), bc2_sqrt be > 0, and
+ * ema_decay lie in [0, 1] (the EMA as in the SGD step). */
 typedef struct y5obb_adam_plan y5obb_adam_plan_t;
 typedef struct {
   float* p;           /* parameter (fp32 master weight), updated in place */
@@ -441,7 +445,7 @@ typedef struct {
 } y5obb_adam_entry;
 int y5obb_adam_ema_plan_create(const y5obb_adam_entry* entries, int n, y5obb_adam_plan_t** out);
 int y5obb_adam_ema_plan_run(const y5obb_adam_plan_t* plan, const float* step_size3, double beta1, double beta2,
-                            float bc2_sqrt, float eps, float ema_decay, void* stream);
+                            float bc2_sqrt, float eps, double ema_decay, void* stream);
 void y5obb_adam_ema_plan_destroy(y5obb_adam_plan_t* plan);
 
 /* ---- tile-merge polygon NMS of the DOTA devkit (CPU form, double precision) ---------------------------------------

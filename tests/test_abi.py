@@ -35,6 +35,18 @@ def test_python_prototypes_cover_the_abi():
     assert L.y5obb_nms_workspace_bytes(1000, 1, 1000) > 1000 * 24
 
 
+def test_abi_version_is_3_with_double_ema_decays():
+    """Version 3: y5obb_sgd_ema_plan_run and y5obb_adam_ema_plan_run take the EMA decay as a double (the kernels form
+    1 - d from it in double, as ModelEMA does), in the header and in the ctypes prototypes alike."""
+    from yolov5_obb_b200 import _lib
+    assert _lib.lib().y5obb_abi_version() == 3
+    txt = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "y5obb.h").read_text(), flags=re.S)
+    for name, at in (("y5obb_sgd_ema_plan_run", 3), ("y5obb_adam_ema_plan_run", 6)):
+        params = re.search(rf"\b{name}\(([^)]*)\)", txt).group(1).split(",")
+        assert params[at].split() == ["double", "ema_decay"], (name, params)
+        assert _lib.PROTOTYPES[name][1][at] is ctypes.c_double, name
+
+
 def test_no_product_import_of_oracle():
     """The product package must never import the oracle (parity would be void)."""
     for p in (ROOT / "yolov5_obb_b200").rglob("*.py"):

@@ -88,6 +88,3 @@ def test_header_and_python_constants_agree():
                  "y5obb_loss_forward_head_f16"):
         assert re.search(rf"\bint {name}\(", h), name
 
-
-def test_abi_version_is_bumped():
-    assert _lib.lib().y5obb_abi_version() == 2

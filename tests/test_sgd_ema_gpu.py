@@ -1,5 +1,6 @@
 """GPU parity of the fused SGD-Nesterov + EMA step (csrc/sgd_ema.cu) against torch.optim.SGD with the reference's parameter
-groups (train.py:148-162) and ModelEMA (utils/torch_utils.py:304-314) over three steps, and of TrainStep's use of it."""
+groups (train.py:148-162) and ModelEMA (utils/torch_utils.py:304-314) over three steps, bit for bit, and of TrainStep's use
+of it (tests/test_sgd_exact_gpu.py checks the same at the edges)."""
 import copy
 import os
 
@@ -41,10 +42,11 @@ def test_fused_step_matches_torch_sgd_and_ema():
         fused.step(lr, mom, ema.decay(ema.updates))
     torch.cuda.synchronize()
     for (n, a), b in zip(m.named_parameters(), ref.parameters()):
-        assert torch.allclose(a, b, rtol=1e-5, atol=1e-7), n
+        assert torch.equal(a, b), n
+        assert torch.equal(fused.mom[a], opt.state[b]["momentum_buffer"]), n
     for (k, a), b in zip(ema.ema.state_dict().items(), ema_ref.ema.state_dict().values()):
         if a.dtype.is_floating_point:
-            assert torch.allclose(a, b, rtol=1e-5, atol=1e-7), k
+            assert torch.equal(a, b), k
 
 
 def test_train_step_fused_equals_torch_path():

@@ -69,11 +69,11 @@ PROTOTYPES = {
     "y5obb_wgrad_schedule": (c_int, [c_void_p] + [ctypes.POINTER(c_int)] * 14),
     "y5obb_wgrad_destroy": (None, [c_void_p]),
     "y5obb_sgd_ema_plan_create": (c_int, [c_void_p, c_int, ctypes.POINTER(c_void_p)]),
-    "y5obb_sgd_ema_plan_run": (c_int, [c_void_p, c_void_p, c_float, c_float, c_int, c_void_p]),
+    "y5obb_sgd_ema_plan_run": (c_int, [c_void_p, c_void_p, c_float, ctypes.c_double, c_int, c_void_p]),
     "y5obb_sgd_ema_plan_destroy": (None, [c_void_p]),
     "y5obb_adam_ema_plan_create": (c_int, [c_void_p, c_int, ctypes.POINTER(c_void_p)]),
-    "y5obb_adam_ema_plan_run": (c_int, [c_void_p, c_void_p, ctypes.c_double, ctypes.c_double, c_float, c_float, c_float,
-                                        c_void_p]),
+    "y5obb_adam_ema_plan_run": (c_int, [c_void_p, c_void_p, ctypes.c_double, ctypes.c_double, c_float, c_float,
+                                        ctypes.c_double, c_void_p]),
     "y5obb_adam_ema_plan_destroy": (None, [c_void_p]),
     "y5obb_poly_nms_workspace_bytes": (c_size_t, [c_int64]),
     "y5obb_poly_nms_f64": (c_int, [c_void_p, c_int64, ctypes.c_double, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

@@ -1176,7 +1176,7 @@ using namespace y5obb;
 
 extern "C" {
 
-int y5obb_abi_version(void) { return 2; }
+int y5obb_abi_version(void) { return 3; }
 int y5obb_last_cuda_error(void) { return g_last_cuda_error; }
 const char* y5obb_build_info(void) { return "liby5obb sm_90a " __DATE__ " " __TIME__; }
 

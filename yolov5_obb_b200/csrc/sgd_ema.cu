@@ -6,9 +6,10 @@
 //                                                 g' = g + wd * p;  m = lerp(m, g', 1 - beta1);  v = beta2 * v + (1 - beta2) g'^2;
 //                                                 p += step_size * m / (sqrt(v) / bc2_sqrt + eps)
 //   utils/torch_utils.py:304-314                  ema = d * ema + (1 - d) * p  for every floating-point state_dict entry
-// tests/test_sgd_ema_gpu.py: equal to torch.optim.SGD + ModelEMA over three steps; train_step.TrainStep uses it whenever every
-// batch ends with an optimizer step (it replaces about 60 multi-tensor launches, 0.6 ms per yolov5m step).
-// tests/test_adam_ema_gpu.py: parameters and moments bit-equal to torch.optim.Adam over five steps.
+// Every op is one _rn intrinsic rounded as torch rounds it, so parameters, momentum buffers, moments and EMA are bit-equal to
+// torch.optim.SGD / torch.optim.Adam's foreach steps and ModelEMA.update's per-tensor ops (tests/test_sgd_exact_gpu.py,
+// tests/test_adam_ema_gpu.py).  train_step.TrainStep uses it whenever every batch ends with an optimizer step (it replaces
+// about 60 multi-tensor launches, 0.6 ms per yolov5m step).
 // HBM-bound: SGD 16 B read + 12 B written per parameter element, Adam 20 B read + 16 B written.
 #include <algorithm>
 #include <vector>
@@ -50,7 +51,8 @@ struct TablePlan {
 
 struct SgdStep {
   float lr[3];
-  float momentum, ema_decay;
+  float momentum;
+  float ema_d, ema_c;      // fp32(d) and fp32(1 - d), 1 - d formed in double
   int first_step;
 };
 
@@ -58,7 +60,8 @@ struct AdamStep {
   float step_size[3];      // -lr / (1 - beta1^t) per group
   float lerp_w;            // 1 - beta1
   float beta2, one_minus_beta2;
-  float bc2_sqrt, eps, ema_decay;
+  float bc2_sqrt, eps;
+  float ema_d, ema_c;      // as SgdStep
 };
 
 // The entry that holds global element i (entries are ordered by `first`).
@@ -72,11 +75,10 @@ __device__ __forceinline__ K find_entry(const K* __restrict__ table, int n, long
   return table[lo];
 }
 
-// ModelEMA.update for one element: v *= d; v += (1 - d) * p, evaluated as fma(v, d, (1 - d) * p) with 1 - d in fp32 (the
-// contraction nvcc chose for the SGD kernel's `d * v + (1 - d) * p`, written out so that both kernels keep it).  ModelEMA's
-// foreach pair rounds v * d first instead: the two differ in the last bits (tests/test_sgd_ema_gpu.py's tolerance).
-__device__ __forceinline__ void ema_update(float* ema, long long j, float p, float d) {
-  if (ema) ema[j] = __fmaf_rn(ema[j], d, __fmul_rn(__fsub_rn(1.0f, d), p));
+// ModelEMA.update for one element, as the reference's per-tensor ops round it on CUDA: v *= d (fp32(d)), then
+// v += (1 - d) * p, where the product is its own rounded op with 1 - d formed in double and read as fp32.
+__device__ __forceinline__ void ema_update(float* ema, long long j, float p, float d, float c) {
+  if (ema) ema[j] = __fadd_rn(__fmul_rn(ema[j], d), __fmul_rn(c, p));
 }
 
 __global__ void k_sgd_ema(const SgdEntryK* __restrict__ table, int n, long long total, SgdStep s) {
@@ -86,14 +88,14 @@ __global__ void k_sgd_ema(const SgdEntryK* __restrict__ table, int n, long long 
     float p = e.p[j];
     if (e.group >= 0) {
       float g = e.g[j];
-      if (e.weight_decay != 0.f) g = g + e.weight_decay * p;          // torch: grad.add(param, alpha=weight_decay)
-      float buf = s.first_step ? g : s.momentum * e.mom[j] + g;        // buf.mul_(momentum).add_(grad)
-      e.mom[j] = buf;
-      g = g + s.momentum * buf;                                         // nesterov: grad.add(buf, alpha=momentum)
-      p = p - s.lr[e.group] * g;                                        // param.add_(grad, alpha=-lr)
+      if (e.weight_decay != 0.f) g = __fmaf_rn(e.weight_decay, p, g);                    // _foreach_add(grads, params, alpha=wd)
+      const float buf = s.first_step ? g : __fadd_rn(__fmul_rn(e.mom[j], s.momentum), g); // _foreach_mul_(bufs, momentum);
+      e.mom[j] = buf;                                                                      // _foreach_add_(bufs, grads)
+      g = __fmaf_rn(s.momentum, buf, g);                                                   // _foreach_add_(grads, bufs, alpha=momentum)
+      p = __fmaf_rn(-s.lr[e.group], g, p);                                                 // _foreach_add_(params, grads, alpha=-lr)
       e.p[j] = p;
     }
-    ema_update(e.ema, j, p, s.ema_decay);
+    ema_update(e.ema, j, p, s.ema_d, s.ema_c);
   }
 }
 
@@ -124,7 +126,7 @@ __global__ void k_adam_ema(const AdamEntryK* __restrict__ table, int n, long lon
       p = __fmaf_rn(__fdiv_rn(m, d), s.step_size[e.group], p);                           // _foreach_addcdiv_(params, m, d, step)
       e.p[j] = p;
     }
-    ema_update(e.ema, j, p, s.ema_decay);
+    ema_update(e.ema, j, p, s.ema_d, s.ema_c);
   }
 }
 
@@ -174,6 +176,7 @@ int y5obb_sgd_ema_plan_create(const y5obb_sgd_entry* entries, int n, y5obb_sgd_p
     const y5obb_sgd_entry& e = entries[i];
     if (!e.p || e.n <= 0 || e.group < -1 || e.group > 2) return Y5OBB_EINVAL;
     if (e.group >= 0 && (!e.g || !e.mom)) return Y5OBB_EINVAL;
+    if (e.group < 0 && !e.ema) return Y5OBB_EINVAL;  // an EMA-only entry without an EMA does nothing: a malformed table
     SgdEntryK& k = h[(size_t)i];
     k.p = e.p;
     k.g = e.g;
@@ -191,16 +194,17 @@ int y5obb_sgd_ema_plan_create(const y5obb_sgd_entry* entries, int n, y5obb_sgd_p
   return rc;
 }
 
-int y5obb_sgd_ema_plan_run(const y5obb_sgd_plan_t* plan, const float* lr3, float momentum, float ema_decay, int first_step,
+int y5obb_sgd_ema_plan_run(const y5obb_sgd_plan_t* plan, const float* lr3, float momentum, double ema_decay, int first_step,
                            void* stream) {
-  if (!plan || !lr3) return Y5OBB_EINVAL;
+  if (!plan || !lr3 || !(momentum >= 0.f) || !(ema_decay >= 0.0 && ema_decay <= 1.0)) return Y5OBB_EINVAL;
   const SgdPlan* p = reinterpret_cast<const SgdPlan*>(plan);
   SgdStep s;
   s.lr[0] = lr3[0];
   s.lr[1] = lr3[1];
   s.lr[2] = lr3[2];
   s.momentum = momentum;
-  s.ema_decay = ema_decay;
+  s.ema_d = (float)ema_decay;
+  s.ema_c = (float)(1.0 - ema_decay);      // ModelEMA: (1 - d) * msd[k], a Python float read as fp32
   s.first_step = first_step;
   k_sgd_ema<<<grid_for(p), 256, 0, (cudaStream_t)stream>>>(p->table, p->n, p->total, s);
   Y5_LAUNCH_CHECK();
@@ -237,9 +241,10 @@ int y5obb_adam_ema_plan_create(const y5obb_adam_entry* entries, int n, y5obb_ada
 }
 
 int y5obb_adam_ema_plan_run(const y5obb_adam_plan_t* plan, const float* step_size3, double beta1, double beta2,
-                            float bc2_sqrt, float eps, float ema_decay, void* stream) {
+                            float bc2_sqrt, float eps, double ema_decay, void* stream) {
   if (!plan || !step_size3) return Y5OBB_EINVAL;
   if (!(beta1 >= 0.0 && beta1 < 1.0) || !(beta2 >= 0.0 && beta2 < 1.0) || !(bc2_sqrt > 0.f)) return Y5OBB_EINVAL;
+  if (!(ema_decay >= 0.0 && ema_decay <= 1.0)) return Y5OBB_EINVAL;
   const AdamPlan* p = reinterpret_cast<const AdamPlan*>(plan);
   AdamStep s;
   s.step_size[0] = step_size3[0];
@@ -250,7 +255,8 @@ int y5obb_adam_ema_plan_run(const y5obb_adam_plan_t* plan, const float* step_siz
   s.one_minus_beta2 = (float)(1.0 - beta2);
   s.bc2_sqrt = bc2_sqrt;
   s.eps = eps;
-  s.ema_decay = ema_decay;
+  s.ema_d = (float)ema_decay;
+  s.ema_c = (float)(1.0 - ema_decay);
   k_adam_ema<<<grid_for(p), 256, 0, (cudaStream_t)stream>>>(p->table, p->n, p->total, s);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;

@@ -128,21 +128,25 @@ class SgdEntry(ctypes.Structure):
 
 
 class FusedSGDEMA:
-    """optimizer.step() + ema.update() of train.py:336-342 as ONE launch (tests/test_sgd_ema_gpu.py: equal to torch.optim.SGD
-    with the reference's parameter groups + ModelEMA within 1e-5 relative over three steps).
+    """optimizer.step() + ema.update() of train.py:336-342 as ONE launch.  Parameters and momentum buffers are bit-equal to
+    torch.optim.SGD(nesterov=True)'s foreach step with the reference's parameter groups, and the EMA to ModelEMA's per-tensor
+    rule (tests/test_sgd_exact_gpu.py).
 
     groups: (g0, g1, g2) parameter lists as train.py:148-156 builds them; grads: {parameter: fp32 gradient tensor} with FIXED
     storage (e.g. views of the backward plan's flat buffer); ema_model: a deep copy whose state_dict mirrors model's.
     step(lr=(lr0, lr1, lr2), momentum, ema_decay) applies torch.optim.SGD(nesterov=True) arithmetic and the EMA rule.
     A parameter with requires_grad False (train.py --freeze) is what torch.optim.SGD makes of a parameter without .grad: it
-    is not moved and has no momentum buffer; the EMA still follows it.  momentum_buffers: {parameter: buffer} to continue
-    from; a trainable parameter without one starts from zeros, which equals torch's clone(grad) on its first step."""
+    is not moved and has no momentum buffer; the EMA still follows it.  state: a mapping {parameter: {'momentum_buffer'}}
+    such as optimizer.state (after a checkpoint's load_state_dict); its buffers are adopted in place (fp32, contiguous, on
+    the parameter's device) and the steps continue from them.  When it holds at least one buffer, a trainable parameter
+    without one starts from zeros: round(0 * momentum + g) is torch's clone(grad) up to the sign of a zero."""
 
-    def __init__(self, model, groups, grads, ema_model=None, weight_decay: float = 0.0, momentum_buffers=None):
+    def __init__(self, model, groups, grads, ema_model=None, weight_decay: float = 0.0, state=None):
         self.device = next(model.parameters()).device
         ema_sd = dict(ema_model.state_dict()) if ema_model is not None else {}
         name_of = {id(p): n for n, p in model.named_parameters()}
         self.mom, ent, self._keep = {}, [], []
+        adopted = 0
         for gi, plist in enumerate(groups):
             for p in plist:
                 e = ema_sd.get(name_of[id(p)])
@@ -153,8 +157,14 @@ class FusedSGDEMA:
                     continue
                 g = grads[p]
                 assert p.dtype == torch.float32 and g.dtype == torch.float32 and p.is_contiguous() and g.is_contiguous()
-                m = momentum_buffers.get(p) if momentum_buffers is not None else None
-                m = torch.zeros_like(p) if m is None else m
+                m = (state.get(p) or {}).get("momentum_buffer") if state is not None else None
+                if m is None:
+                    m = torch.zeros_like(p)
+                else:
+                    if m.dtype != torch.float32 or m.device != p.device or m.shape != p.shape or not m.is_contiguous():
+                        raise ValueError("FusedSGDEMA: adopted momentum buffers must be contiguous fp32 tensors shaped and "
+                                         "placed like their parameter")
+                    adopted += 1
                 self.mom[p] = m
                 ent.append(SgdEntry(p.data_ptr(), g.data_ptr(), m.data_ptr(), e.data_ptr() if e is not None else None, p.numel(),
                                     float(weight_decay) if gi == 1 else 0.0, gi))
@@ -173,7 +183,7 @@ class FusedSGDEMA:
         with torch.cuda.device(self.device):
             rc = _lib.lib().y5obb_sgd_ema_plan_create(arr, len(ent), ctypes.byref(self._h))
         _lib.check(rc, "y5obb_sgd_ema_plan_create")
-        self.steps = 0 if momentum_buffers is None else 1  # adopted buffers already hold a first step
+        self.steps = 1 if adopted else 0  # adopted buffers already hold a first step
 
     def step(self, lr, momentum: float, ema_decay: float = 0.0, stream=None):
         lr3 = (ctypes.c_float * 3)(*[float(v) for v in lr])
@@ -182,6 +192,43 @@ class FusedSGDEMA:
                                                    stream if stream is not None else _lib.stream_ptr(self.device))
         _lib.check(rc, "y5obb_sgd_ema_plan_run")
         self.steps += 1
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            try:
+                _lib.lib().y5obb_sgd_ema_plan_destroy(h)
+            except Exception:
+                pass
+            self._h = None
+
+
+class FusedEMA:
+    """ModelEMA.update alone as ONE launch: a table of EMA-only entries (group -1) of the SGD + EMA kernel, one per
+    (source, ema) pair of fp32 device tensors with FIXED storage.  step(ema_decay) rounds as the reference's per-tensor
+    ops: v *= d; v += (1 - d) * p."""
+
+    def __init__(self, sources, emas):
+        ent, self._keep = [], []
+        for s, e in zip(sources, emas):
+            if s.dtype != torch.float32 or e.dtype != torch.float32 or not s.is_cuda or s.device != e.device or \
+                    s.shape != e.shape or not s.is_contiguous() or not e.is_contiguous():
+                raise ValueError("FusedEMA: sources and EMA copies must be contiguous fp32 device tensors of one shape")
+            ent.append(SgdEntry(s.data_ptr(), None, None, e.data_ptr(), s.numel(), 0.0, -1))
+            self._keep += [s, e]
+        self.device = self._keep[0].device
+        arr = (SgdEntry * len(ent))(*ent)
+        self._h = c_void_p()
+        with torch.cuda.device(self.device):
+            rc = _lib.lib().y5obb_sgd_ema_plan_create(arr, len(ent), ctypes.byref(self._h))
+        _lib.check(rc, "y5obb_sgd_ema_plan_create")
+
+    def step(self, ema_decay: float, stream=None):
+        lr3 = (ctypes.c_float * 3)(0.0, 0.0, 0.0)
+        with torch.cuda.device(self.device):
+            rc = _lib.lib().y5obb_sgd_ema_plan_run(self._h, lr3, 0.0, float(ema_decay), 0,
+                                                   stream if stream is not None else _lib.stream_ptr(self.device))
+        _lib.check(rc, "y5obb_sgd_ema_plan_run")
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -210,8 +257,8 @@ def adam_step_scalars(lr: float, beta1: float, beta2: float, step: float):
 
 class FusedAdamEMA:
     """optimizer.step() of torch.optim.Adam (train.py --adam, train.py:157-163: coupled L2 weight decay, amsgrad off) +
-    ema.update() as ONE launch.  Parameters, exp_avg and exp_avg_sq are bit-equal to torch's foreach step
-    (tests/test_adam_ema_gpu.py); the EMA is the SGD kernel's (equal to ModelEMA within 1e-5 relative).
+    ema.update() as ONE launch.  Parameters, exp_avg and exp_avg_sq are bit-equal to torch's foreach step, and the EMA to
+    ModelEMA's per-tensor rule (tests/test_adam_ema_gpu.py).
 
     groups, grads, ema_model, weight_decay: as FusedSGDEMA (weight decay on group 1 only).  state: a mapping
     {parameter: {'step', 'exp_avg', 'exp_avg_sq'}} such as optimizer.state; where it holds every parameter the moments are

@@ -79,7 +79,10 @@ def multi_scale_max_shape(imgsz: int, gs: int, H: int, W: int):
 
 
 class ModelEMA:
-    """utils/torch_utils.py:284-314: EMA of every floating-point state_dict entry, decay ramp d*(1-exp(-n/2000))."""
+    """utils/torch_utils.py:284-314: EMA of every floating-point state_dict entry, decay ramp d*(1-exp(-n/2000)).
+    update() rounds as the reference's per-tensor `v *= d; v += (1 - d) * msd[k]` does: the product (1 - d) * p is rounded
+    before the add (an alpha add would fuse it into one FMA).  On the device, with fp32 entries, it is one launch of the
+    SGD + EMA kernel over an EMA-only table (train_ops.FusedEMA); elsewhere the same rule as foreach ops."""
 
     def __init__(self, model, decay=0.9999, updates=0):
         engines = getattr(model, "_engines", None)
@@ -93,6 +96,7 @@ class ModelEMA:
         for p in self.ema.parameters():
             p.requires_grad_(False)
         self._pairs = None
+        self._fused = None
 
     def update(self, model):
         with torch.no_grad():
@@ -106,9 +110,17 @@ class ModelEMA:
                         ev.append(v)
                         mv.append(msd[k].detach())
                 self._pairs = (ev, mv)
+                if ev and all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in ev + mv):
+                    from .train_ops import FusedEMA
+                    self._fused = FusedEMA(mv, ev)
+            if self._fused is not None:
+                self._fused.step(d)
+                if hasattr(self.ema, "_bump_generation"):
+                    self.ema._bump_generation()   # written through raw pointers: inference plans must re-fold the EMA
+                return
             ev, mv = self._pairs
             torch._foreach_mul_(ev, d)
-            torch._foreach_add_(ev, mv, alpha=1 - d)
+            torch._foreach_add_(ev, torch._foreach_mul(mv, 1 - d))
 
 
 class TrainStep:
@@ -191,8 +203,8 @@ class TrainStep:
         self.optimizer.zero_grad(set_to_none=True)
         # optimizer.step() + ema.update() as ONE kernel (csrc/sgd_ema.cu, SURVEY 8f rank 1) whenever every batch ends with an
         # optimizer step (accumulate == 1: the gradient of the step is exactly the backward plan's flat buffer).  With gradient
-        # accumulation torch.optim.SGD / Adam + the foreach EMA below stay in charge.  Y5OBB_FUSED_SGD=0 forces the torch path
-        # for either optimizer.
+        # accumulation torch.optim.SGD / Adam + ModelEMA.update stay in charge.  Y5OBB_FUSED_SGD=0 forces the torch path for
+        # either optimizer.
         import os
         self._fused = None
         self._fused_state = None
@@ -353,8 +365,8 @@ class TrainStep:
         learning rates / momentum are taken from optimizer.param_groups every step, so warm-up schedules that edit them
         (train.py:305-316) keep working; the momentum buffers are registered in optimizer.state for checkpoints.
         Adam: lr, betas and eps are read the same way, and optimizer.state holds torch's exp_avg / exp_avg_sq / step, which
-        the kernel updates in place.  optimizer.load_state_dict() replaces optimizer.state, so a new state object means a
-        checkpoint was loaded: the table is rebuilt on the loaded tensors."""
+        the kernel updates in place.  optimizer.load_state_dict() replaces optimizer.state, so for either optimizer a new
+        state object means a checkpoint was loaded: the table is rebuilt on the loaded tensors."""
         from .train_ops import FusedAdamEMA, FusedSGDEMA
         model = self.model
         plan = model._last_train_engine._bwd
@@ -374,22 +386,24 @@ class TrainStep:
                 for p, s in self._fused.state.items():
                     opt.state[p] = s
                 self._fused_state = opt.state
-        elif rebuild:
+        elif rebuild or self._fused_state is not opt.state:
             groups = [g["params"] for g in opt.param_groups]
-            self._fused = FusedSGDEMA(model, groups, plan.pgrad, ema,
-                                      weight_decay=self.hyp["weight_decay"], momentum_buffers=getattr(self, "_mom", None))
-            # (the buffers of parameters frozen since are kept: torch's SGD resumes from them after an unfreeze)
-            self._mom = dict(getattr(self, "_mom", None) or {})
-            self._mom.update(self._fused.mom)
+            # adopts the buffers optimizer.state holds: a loaded checkpoint's, or this run's (the buffers of parameters frozen
+            # since stay there, and torch's SGD resumes from them after an unfreeze)
+            self._fused = FusedSGDEMA(model, groups, plan.pgrad, ema, weight_decay=self.hyp["weight_decay"], state=opt.state)
             self._fused_plan, self._fused_flags = key, plan.trainable
             for p, m in self._fused.mom.items():
                 opt.state[p]["momentum_buffer"] = m
+            self._fused_state = opt.state
         g = opt.param_groups
         if self.adam:
             betas, eps = g[0]["betas"], g[0]["eps"]
             if any(tuple(x["betas"]) != tuple(betas) or x["eps"] != eps for x in g[1:]):
                 raise ValueError("the fused Adam step needs one (betas, eps) for every parameter group; "
                                  "set Y5OBB_FUSED_SGD=0 to step per group with torch.optim.Adam")
+        elif any(x["momentum"] != g[0]["momentum"] for x in g[1:]):
+            raise ValueError("the fused SGD step needs one momentum for every parameter group; "
+                             "set Y5OBB_FUSED_SGD=0 to step per group with torch.optim.SGD")
         d = 0.0
         if self.ema is not None:
             self.ema.updates += 1
