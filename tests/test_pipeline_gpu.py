@@ -48,6 +48,63 @@ def test_pipeline_equals_blocking_calls(slots, fused):
     assert pipe.h2d_bytes == sum(x.numel() for x in batches)
 
 
+class _NoHint(dict):
+    """A general._CAP_HINT that never learns: every async NMS starts from the optimistic capacity again."""
+
+    def __setitem__(self, key, value):
+        pass
+
+
+def test_overflowed_batches_are_rerun_in_both_forms(monkeypatch):
+    """conf_thres=0 with multi_label: every (anchor, class) pair of a 2 x 256^2 batch is a candidate, 2 * 4032 * 15 = 120,960
+    against the optimistic capacity of 65,536, so the async NMS of every batch overflows and the pipeline re-runs it blocking.
+    Both forms, two slots on one pipeline: each yielded batch must still equal the blocking calls, in order."""
+    from tests.letterboxgen import synth_image
+    from yolov5_obb_b200 import general
+    from yolov5_obb_b200 import letterbox as lb
+    from yolov5_obb_b200 import pipeline as P
+    monkeypatch.setattr(general, "_CAP_HINT", _NoHint())
+    nms = general.non_max_suppression_obb
+    reruns = []
+
+    def counting_nms(pred, **kw):
+        reruns.append(kw.get("return_packed") is True)
+        return nms(pred, **kw)
+
+    monkeypatch.setattr(P, "non_max_suppression_obb", counting_nms)
+    m = build_mirror("n", nc=15, seed=0, obj_bias=1.0, cls_bias=-1.0, det_gain=6.0).to(DEV)
+    kw = dict(conf_thres=0.0, iou_thres=0.45, multi_label=True, max_det=300)
+    pipe = P.DetectPipeline(m, device=DEV, slots=2, **kw)
+
+    batches = [synth_tiles(2, 256, seed=s).pin_memory() for s in range(1, 5)]
+    want = [[d.cpu() for d in nms(m.detect_records(xb.to(DEV)), **kw)] for xb in batches]
+    got = list(pipe(iter(batches)))
+    assert sum(reruns) == len(batches) == len(got)
+    for g, w in zip(got, want):
+        assert len(g) == len(w) and all(torch.equal(a, b) for a, b in zip(g, w))
+
+    images = [synth_image(256, 256, 30 + k) for k in range(8)]
+    order, shapes = lb.rect_batch_shapes([(256, 256)] * len(images), 2, 256, 32, 0.0)
+    want = [None] * len(images)
+    for b, (Hp, Wp) in enumerate(shapes.tolist()):
+        idx = [int(k) for k in order[2 * b:2 * b + 2]]
+        places = [lb.place_rect(256, 256, 256, (Hp, Wp)) for _ in idx]
+        batch = lb.pack_batch([images[k] for k in idx], places, Hp, Wp)
+        eng = m.records_plan((2, 3, Hp, Wp), DEV)
+        lb.letterbox_s2d(batch.host[:batch.nbytes].to(DEV), batch, eng.x_s2d, 1)
+        packed, counts = nms(general.DetectRecords(eng.forward_s2d(), eng.nc, eng.half), return_packed=True, **kw)
+        pad_gain = torch.tensor([p.pad_gain for p in places], dtype=torch.float32, device=DEV)
+        polys = lb.scale_polys_batched(packed, torch.tensor(counts, device=DEV), pad_gain).cpu()
+        for i, k in enumerate(idx):
+            want[k] = (polys[i, :counts[i]], packed[i, :counts[i]].cpu())
+    reruns.clear()
+    got = list(pipe.run_images(images, img_size=256, stride=32, auto=False, batch_size=2))
+    assert sum(reruns) == len(shapes) and len(got) == len(images)
+    assert sum(r.shape[0] for _, r in want) > 0
+    for g, (poly, rows) in zip(got, want):
+        assert torch.equal(g.rows, rows) and torch.equal(g.polys, poly)
+
+
 def test_submit_fork_join_device_resident():
     """DetectPipeline.submit: device-resident batches round-robin over the slot streams, bracketed by fork() / join(); each
     slot's last result equals the blocking call on that batch (distinct batches, so a slot mix-up cannot pass)."""

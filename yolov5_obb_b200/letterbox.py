@@ -5,7 +5,8 @@ The reference does all of it on the CPU, per image: cv2.resize + copyMakeBorder 
 utils/datasets.py:217-229 and :585-590,662-663,702-720) before the forward and rbox2poly + scale_polys after NMS
 (detect.py:129-147, val.py:226-232).  Here only the O(width + height) geometry stays on the host: letterbox_geometry,
 load_image_size and rect_batch_shapes return the reference's values, pack_batch ships the decoded images as they are with one
-descriptor and two coefficient tables each, and y5obb_letterbox_s2d_u8 writes the stem input of the whole batch.  The tables
+descriptor and two coefficient tables each, and y5obb_letterbox_s2d_u8 writes the stem input of the whole batch
+(letterboxed_records runs it and the records plan for DetectPipeline.run_images and the Validator's raw form).  The tables
 are formed in the float types OpenCV uses (DESIGN.md section 4), so the resampled bytes are OpenCV's."""
 import functools
 from typing import Optional, Sequence, Tuple
@@ -14,6 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .general import DetectRecords
 
 LINEAR, AREA = "linear", "area"
 MODE_COPY, MODE_LINEAR, MODE_AREA_INT, MODE_AREA = 0, 1, 2, 3   # Y5OBB_LB_*
@@ -315,6 +317,16 @@ def letterbox_s2d(dev_buf: torch.Tensor, batch: PackedBatch, x_s2d: torch.Tensor
         _lib.check(getattr(_lib.lib(), name)(base + batch.src_off, batch.src_bytes, base, batch.host.data_ptr(),
                                              batch.desc_bytes, batch.B, batch.Hp, batch.Wp, x_s2d.data_ptr(), pad_cols,
                                              _lib.stream_ptr(dev_buf.device)), name)
+
+
+def letterboxed_records(model, dev_buf: torch.Tensor, batch: PackedBatch, device, slot: int = 0):
+    """Runs a packed batch through `model`'s records plan for the batch's shape and `slot`, on the current stream:
+    letterbox_s2d writes the plan's stem input from dev_buf (batch.host[:batch.nbytes] on the device), then forward_s2d.
+    -> (general.DetectRecords, the per-image (pad_x, pad_y, gain) fp32 table for scale_polys_batched, a view of dev_buf)."""
+    eng = model.records_plan((batch.B, 3, batch.Hp, batch.Wp), device, slot)
+    letterbox_s2d(dev_buf, batch, eng.x_s2d, 1)
+    pad_gain = dev_buf[batch.pad_gain_off:batch.pad_gain_off + 12 * batch.B].view(torch.float32)
+    return DetectRecords(eng.forward_s2d(), eng.nc, eng.half), pad_gain
 
 
 def scale_polys_batched(rows: torch.Tensor, counts: torch.Tensor, pad_gain: torch.Tensor) -> torch.Tensor:

@@ -6,19 +6,21 @@ val.py:183-207 (pre-process, inference, NMS), software-pipelined:
   leave SMs idle, and the NMS stage is a chain of small latency-bound kernels: a second batch on another stream fills both
   (tools/time_streams.py compares slot counts).  Results are bit-identical to the blocking calls: the same kernels run on the same data, only
   their interleaving changes.
-* the host->device copy of batch i+1 runs on a copy stream while batch i computes (max(2, slots) device input buffers,
-  event-ordered), and the device->host copy of batch i's detections is asynchronous, so the host turns batch i-slots into
-  per-image tensors while the GPU works on the batches after it (no stream is drained inside the loop).
+* the host->device copy of batch i+1 runs on a copy stream while batch i computes (max(2, slots) grow-only device input
+  buffers, event-ordered), and the device->host copy of batch i's detections into a ring of slots + 1 pinned result slots is
+  asynchronous, so the host turns batch i-slots into per-image tensors while the GPU works on the batches after it (no stream
+  is drained inside the loop, except to re-run a batch whose NMS candidates overflowed the optimistic capacity).
 
-`run_images` is the same pipeline for decoded images of any size (detect.py's `LoadImages`, val.py's rect loader): the upload
-is the raw packed batch, csrc/letterbox.cu writes the plan's stem input, and the detections come back as polygons in source
-pixels (letterbox.py)."""
+`__call__` (letterboxed tensors) and `run_images` (decoded images of any size: detect.py's `LoadImages`, val.py's rect loader)
+run that one loop and differ only in what it uploads, how a batch's records are produced and what is read back: `run_images`
+uploads the raw packed batch, csrc/letterbox.cu writes the plan's stem input, and the detections come back with polygons in
+source pixels (letterbox.py)."""
 from typing import Iterable, Iterator, List, NamedTuple, Optional
 
 import torch
 
 from . import letterbox as lb
-from .general import DetectRecords, non_max_suppression_obb
+from .general import non_max_suppression_obb
 
 
 class ImageDetections(NamedTuple):
@@ -67,10 +69,8 @@ class DetectPipeline:
         self._copied = [torch.cuda.Event() for _ in range(self.n_in)]
         self._consumed = [torch.cuda.Event() for _ in range(self.n_in)]
         self._reader = [0] * self.n_in          # the slot whose stream read the buffer last
+        self._raw_host = [None] * self.n_in     # run_images: grow-only pinned host buffers of the packed batches
         self._hslots = None
-        self._raw_dev = [None] * self.n_in      # run_images: grow-only device / pinned host buffers of the packed batches
-        self._raw_host = [None] * self.n_in
-        self._raw_hslots = None
         self._next = 0
         self.h2d_bytes = 0
         self.d2h_bytes = 0
@@ -98,6 +98,10 @@ class DetectPipeline:
             ev.record(st)
             cur.wait_event(ev)
 
+    def _predict(self, x: torch.Tensor, slot: int = 0):
+        """The compact records (fused) or Model.forward's prediction tensor of a device batch, on the current stream."""
+        return self.model.detect_records(x, slot=slot) if self.fused else self.model(x)[0]
+
     def submit(self, x_dev: torch.Tensor, slot: Optional[int] = None):
         """One batch that is already on the device -> (packed [B, max_det, 7], counts int64 [B + 1], cap), device tensors
         (no host read; non_max_suppression_obb's `return_packed="async"` form).  Runs on the slot's stream - round-robin
@@ -107,88 +111,15 @@ class DetectPipeline:
             slot = self._next
             self._next = (self._next + 1) % self.slots
         with torch.cuda.stream(self._stream(slot)):
-            pred = self.model.detect_records(x_dev, slot=slot) if self.fused else self.model(x_dev)[0]
-            return non_max_suppression_obb(pred, return_packed="async", **self.kw)
+            return non_max_suppression_obb(self._predict(x_dev, slot), return_packed="async", **self.kw)
 
-    # ------------------------------------------------------------------ host-to-host form
-    def _host_slot(self, j, B, max_det):
-        hs = self._hslots
-        if hs is None or hs[0][0].shape[0] != B or hs[0][0].shape[1] != max_det:
-            self._hslots = hs = [(torch.empty((B, max_det, 7), dtype=torch.float32).pin_memory(),
-                                  torch.empty(B + 1, dtype=torch.int64).pin_memory(), torch.cuda.Event())
-                                 for _ in range(self.slots + 1)]
-        return hs[j]
-
-    def _upload(self, j: int, x_host: torch.Tensor, first_use: bool) -> None:
-        if self._bufs[j] is None or self._bufs[j].shape != x_host.shape or self._bufs[j].dtype != x_host.dtype:
-            if not first_use:
-                self._stream(self._reader[j]).synchronize()   # (shape change mid-stream: the old buffer may still be read)
-            self._bufs[j] = torch.empty(x_host.shape, dtype=x_host.dtype, device=self.device)
-            first_use = True
-        with torch.cuda.stream(self.copy_stream):
-            if not first_use:
-                self.copy_stream.wait_event(self._consumed[j])  # the engine finished reading this buffer
-            self._bufs[j].copy_(x_host, non_blocking=True)
-            self._copied[j].record(self.copy_stream)
-        self.h2d_bytes += x_host.numel() * x_host.element_size()
-
+    # ------------------------------------------------------------------ host-to-host forms
     def __call__(self, host_batches: Iterable[torch.Tensor]) -> Iterator[List[torch.Tensor]]:
         """host_batches: pinned uint8 (0..255) or float (0..1) tensors [B,3,H,W].  Yields, per batch and in order, the list
         of per-image detections [n,7] (cx, cy, l, s, theta, conf, cls) as HOST tensors."""
-        it = iter(host_batches)
-        cur = next(it, None)
-        if cur is None:
-            return
-        N, NB = self.slots, self.n_in
-        used = [False] * NB
-        self.fork()
-        self._upload(0, cur, True)
-        used[0] = True
-        i = 0
-        pending = []
-        while cur is not None:
-            slot, j, jn, hs = schedule(i, N, NB)
-            nxt = next(it, None)
-            if nxt is not None:   # (its previous user, batch i + 1 - NB <= i - 1, has been queued: _consumed[jn] is its event)
-                self._upload(jn, nxt, not used[jn])
-                used[jn] = True
-            compute = self._stream(slot)
-            with torch.cuda.stream(compute):
-                compute.wait_event(self._copied[j])
-                pred = self.model.detect_records(self._bufs[j], slot=slot) if self.fused else self.model(self._bufs[j])[0]
-                self._consumed[j].record(compute)  # the layout pass has consumed the input by now (stream order)
-                self._reader[j] = slot
-                packed, counts, cap = non_max_suppression_obb(pred, return_packed="async", **self.kw)
-                # batch i - (N + 1), the previous user of this pinned slot, was handed to the caller before this point
-                hout, hcnt, ev = self._host_slot(hs, packed.shape[0], packed.shape[1])
-                hout.copy_(packed, non_blocking=True)   # D2H of this batch's result, one copy; nobody waits for it here
-                hcnt.copy_(counts, non_blocking=True)
-                ev.record(compute)
-            self.d2h_bytes += packed.numel() * 4 + counts.numel() * 8
-            pending.append((hout, hcnt, ev, cap, cur))
-            if len(pending) > N:       # N batches stay queued behind the one the host waits for
-                yield self._finish(pending.pop(0))
-            cur = nxt
-            i += 1
-        while pending:
-            yield self._finish(pending.pop(0))
-        self.join()
+        return self._run(host_batches, lambda x, j: (x, None), lambda x, _, slot: (self._predict(x, slot), None),
+                         lambda x, rows, polys, counts: [rows[b, :k].clone() for b, k in enumerate(counts)])
 
-    def _finish(self, pending):
-        hout, hcnt, ev, cap, x_host = pending
-        ev.synchronize()
-        c = hcnt.tolist()
-        B = len(c) - 1
-        if c[B] > cap or c[B] < 0 or any(k < 0 for k in c[:B]):  # rare: more candidates than the optimistic capacity -> re-run, blocking
-            torch.cuda.synchronize(self.device)   # the slots' plans are shared with batches in flight: drain them first
-            xd = x_host.to(self.device)
-            pred = self.model.detect_records(xd) if self.fused else self.model(xd)[0]
-            packed, counts = non_max_suppression_obb(pred, return_packed=True, **self.kw)
-            host = packed.cpu()
-            return [host[b, :k].clone() for b, k in enumerate(counts)]
-        return [hout[b, :k].clone() for b, k in enumerate(c[:B])]
-
-    # ------------------------------------------------------------------ decoded images of any size
     def run_images(self, images, img_size: int = 1024, stride: Optional[int] = None, auto: bool = True, batch_size: int = 1,
                    pad: float = 0.0) -> Iterator[ImageDetections]:
         """images: uint8 [H, W, 3] BGR arrays (numpy or CPU tensors, as cv2.imread returns them) of any sizes.  Yields one
@@ -232,112 +163,127 @@ class DetectPipeline:
                     Hp, Wp = int(shapes[i][0]), int(shapes[i][1])
                     yield idx, [ims[k] for k in idx], [lb.place_rect(ims[k].shape[0], ims[k].shape[1], img_size, (Hp, Wp))
                                                        for k in idx], Hp, Wp
+
+        def pack(item, j):
+            _, ims_b, places, Hp, Wp = item
+            if j is None:
+                batch = lb.pack_batch(ims_b, places, Hp, Wp)
+            else:
+                self._copied[j].synchronize()   # the previous upload from this pinned buffer (n_in batches ago) has completed
+                batch = lb.pack_batch(ims_b, places, Hp, Wp, self._raw_host[j])
+                self._raw_host[j] = batch.host
+            return batch.host[:batch.nbytes], batch
+
+        def emit(item, rows, polys, counts):
+            idx, _, places, _, _ = item
+            out = []
+            for b, k in enumerate(counts):
+                r = rows[b, :k].clone()
+                out.append(ImageDetections(polys[b, :k].clone(), r[:, 5], r[:, 6], r, places[b].shapes))
+            return idx, out
+
         ready, nxt_out = {}, 0
-        for idx, dets in self._run_raw(batches()):
+        for idx, dets in self._run(batches(), pack,
+                                   lambda buf, batch, slot: lb.letterboxed_records(self.model, buf, batch, self.device, slot),
+                                   emit):
             ready.update(zip(idx, dets))
             while nxt_out in ready:
                 yield ready.pop(nxt_out)
                 nxt_out += 1
 
-    def _pack(self, j: int, used: bool, raw):
-        idx, ims, places, Hp, Wp = raw
-        if used:
-            self._copied[j].synchronize()   # the previous upload from this pinned buffer (n_in batches ago) has completed
-        batch = lb.pack_batch(ims, places, Hp, Wp, self._raw_host[j])
-        self._raw_host[j] = batch.host
-        return batch
-
-    def _upload_raw(self, j: int, batch, first_use: bool) -> None:
-        buf = self._raw_dev[j]
-        if buf is None or buf.numel() < batch.nbytes:
-            if buf is not None and not first_use:
-                self._stream(self._reader[j]).synchronize()   # (the smaller buffer may still be read)
-            buf = self._raw_dev[j] = torch.empty(int(batch.nbytes * 1.25) + 4096, dtype=torch.uint8, device=self.device)
-            first_use = True
-        with torch.cuda.stream(self.copy_stream):
-            if not first_use:
-                self.copy_stream.wait_event(self._consumed[j])
-            buf[:batch.nbytes].copy_(batch.host[:batch.nbytes], non_blocking=True)
-            self._copied[j].record(self.copy_stream)
-        self.h2d_bytes += batch.nbytes
-
-    def _raw_host_slot(self, j: int, B: int, max_det: int):
-        hs = self._raw_hslots
-        if hs is None or hs[0][0].shape[0] < B or hs[0][0].shape[1] != max_det:
-            self._raw_hslots = hs = [(torch.empty((B, max_det, 7), dtype=torch.float32).pin_memory(),
-                                      torch.empty((B, max_det, 8), dtype=torch.float32).pin_memory(),
-                                      torch.empty(B + 1, dtype=torch.int64).pin_memory(), torch.cuda.Event())
-                                     for _ in range(self.slots + 1)]
-        return hs[j]
-
-    def _detect_raw(self, buf, batch, slot: int):
-        """letterbox kernel -> records plan -> (records, per-image (pad_x, pad_y, gain) on the device)."""
-        eng = self.model.records_plan((batch.B, 3, batch.Hp, batch.Wp), self.device, slot)
-        lb.letterbox_s2d(buf, batch, eng.x_s2d, 1)
-        pad_gain = buf[batch.pad_gain_off:batch.pad_gain_off + 12 * batch.B].view(torch.float32)
-        return DetectRecords(eng.forward_s2d(), eng.nc, eng.half), pad_gain
-
-    def _run_raw(self, raw_batches):
-        """The loop of __call__ for packed raw batches: yields (input indices, [ImageDetections]) per batch, in batch order."""
-        it = iter(raw_batches)
+    def _run(self, items, pack, detect, emit):
+        """The pipelined loop of both host-to-host forms.  For each batch `item` the form supplies
+        * pack(item, j) -> (host tensor to upload, aux), in the pinned host buffer that goes with device input buffer j, or
+          in one of its own when j is None (the blocking re-run);
+        * detect(device copy, aux, slot) -> (what non_max_suppression_obb takes, per-image (pad_x, pad_y, gain) fp32 on the
+          device or None), on the current stream; with the pad / gain table the polygons in source pixels come back too;
+        * emit(item, rows, polys, counts) -> what is yielded for the batch, from host rows [>= B, max_det, 7], polygons
+          [>= B, max_det, 8] (meaningful only with the pad / gain table) and the B per-image row counts."""
+        it = iter(items)
         cur = next(it, None)
         if cur is None:
             return
         N, NB = self.slots, self.n_in
         used = [False] * NB
         self.fork()
-        cur_b = self._pack(0, False, cur)
-        self._upload_raw(0, cur_b, True)
+        staged = self._upload(0, *pack(cur, 0), True)
         used[0] = True
         i = 0
         pending = []
         while cur is not None:
             slot, j, jn, hs = schedule(i, N, NB)
-            nxt = next(it, None)
-            nxt_b = None
-            if nxt is not None:
-                nxt_b = self._pack(jn, used[jn], nxt)
-                self._upload_raw(jn, nxt_b, not used[jn])
+            nxt, nxt_staged = next(it, None), None
+            if nxt is not None:   # (its previous user, batch i + 1 - NB <= i - 1, has been queued: _consumed[jn] is its event)
+                nxt_staged = self._upload(jn, *pack(nxt, jn), not used[jn])
                 used[jn] = True
             compute = self._stream(slot)
-            B = cur_b.B
             with torch.cuda.stream(compute):
                 compute.wait_event(self._copied[j])
-                rec, pad_gain = self._detect_raw(self._raw_dev[j], cur_b, slot)
-                packed, counts, cap = non_max_suppression_obb(rec, return_packed="async", **self.kw)
-                polys = lb.scale_polys_batched(packed, counts, pad_gain)
-                self._consumed[j].record(compute)   # (the polygon kernel read the batch's pad / gain table)
+                rec, pad_gain = detect(*staged, slot)
+                self._consumed[j].record(compute)  # the layout pass has consumed the input by now (stream order)
                 self._reader[j] = slot
-                hout, hpoly, hcnt, ev = self._raw_host_slot(hs, B, packed.shape[1])
-                hout[:B].copy_(packed, non_blocking=True)
-                hpoly[:B].copy_(polys, non_blocking=True)
+                packed, counts, cap = non_max_suppression_obb(rec, return_packed="async", **self.kw)
+                B, polys = packed.shape[0], None
+                if pad_gain is not None:
+                    polys = lb.scale_polys_batched(packed, counts, pad_gain)
+                    self._consumed[j].record(compute)   # re-recorded: this kernel reads the pad / gain table from the input
+                # batch i - (N + 1), the previous user of this pinned slot, was handed to the caller before this point
+                hout, hpoly, hcnt, ev = self._host_slot(hs, B, polys is not None)
+                hout[:B].copy_(packed, non_blocking=True)   # D2H of this batch's result; nobody waits for it here
+                if polys is not None:
+                    hpoly[:B].copy_(polys, non_blocking=True)
                 hcnt[:B + 1].copy_(counts, non_blocking=True)
                 ev.record(compute)
-            self.d2h_bytes += packed.numel() * 4 + polys.numel() * 4 + counts.numel() * 8
-            pending.append((hout, hpoly, hcnt, ev, cap, cur))
-            if len(pending) > N:
-                yield self._finish_raw(pending.pop(0))
-            cur, cur_b = nxt, nxt_b
+            self.d2h_bytes += packed.numel() * 4 + counts.numel() * 8 + (0 if polys is None else polys.numel() * 4)
+            pending.append((cur, B, hout, hpoly, hcnt, ev, cap))
+            if len(pending) > N:       # N batches stay queued behind the one the host waits for
+                yield self._finish(pending.pop(0), pack, detect, emit)
+            cur, staged = nxt, nxt_staged
             i += 1
         while pending:
-            yield self._finish_raw(pending.pop(0))
+            yield self._finish(pending.pop(0), pack, detect, emit)
         self.join()
 
-    def _finish_raw(self, pending):
-        hout, hpoly, hcnt, ev, cap, (idx, ims, places, Hp, Wp) = pending
+    def _upload(self, j: int, src: torch.Tensor, aux, first_use: bool):
+        """H2D of `src` into device input buffer j on the copy stream, once the previous batch's reader has consumed it ->
+        (the device copy, aux).  The buffer is grow-only bytes, so batches of varying sizes rarely re-allocate it."""
+        buf, n = self._bufs[j], src.numel() * src.element_size()
+        if buf is None or buf.numel() < n:
+            if not first_use:
+                self._stream(self._reader[j]).synchronize()   # (the smaller buffer may still be read)
+            buf = self._bufs[j] = torch.empty(int(n * 1.25) + 4096, dtype=torch.uint8, device=self.device)
+            first_use = True
+        dst = buf[:n].view(src.dtype).view(src.shape)
+        with torch.cuda.stream(self.copy_stream):
+            if not first_use:
+                self.copy_stream.wait_event(self._consumed[j])  # the engine finished reading this buffer
+            dst.copy_(src, non_blocking=True)
+            self._copied[j].record(self.copy_stream)
+        self.h2d_bytes += n
+        return dst, aux
+
+    def _host_slot(self, k: int, B: int, polys: bool):
+        """Pinned result slot k of the ring of slots + 1: (rows, polygons or None, counts, the event of their D2H copy),
+        grow-only in the batch size."""
+        hs = self._hslots
+        if hs is None or hs[0][0].shape[0] < B or (polys and hs[0][1] is None):
+            max_det = self.kw["max_det"]
+            self._hslots = hs = [(torch.empty((B, max_det, 7), dtype=torch.float32).pin_memory(),
+                                  torch.empty((B, max_det, 8), dtype=torch.float32).pin_memory() if polys else None,
+                                  torch.empty(B + 1, dtype=torch.int64).pin_memory(), torch.cuda.Event())
+                                 for _ in range(self.slots + 1)]
+        return hs[k]
+
+    def _finish(self, pending, pack, detect, emit):
+        item, B, hout, hpoly, hcnt, ev, cap = pending
         ev.synchronize()
-        B = len(idx)
         c = hcnt[:B + 1].tolist()
-        if c[B] > cap or c[B] < 0 or any(k < 0 for k in c[:B]):  # rare: NMS capacity overflow -> re-run, blocking
-            torch.cuda.synchronize(self.device)
-            batch = lb.pack_batch(ims, places, Hp, Wp)
-            buf = batch.host[:batch.nbytes].to(self.device)
-            rec, pad_gain = self._detect_raw(buf, batch, 0)
-            packed, counts = non_max_suppression_obb(rec, return_packed=True, **self.kw)
-            cdev = torch.tensor(counts, dtype=torch.int64).to(self.device)
-            hout, hpoly, c = packed.cpu(), lb.scale_polys_batched(packed, cdev, pad_gain).cpu(), counts
-        out = []
-        for b, k in enumerate(c[:B]):
-            rows = hout[b, :k].clone()
-            out.append(ImageDetections(hpoly[b, :k].clone(), rows[:, 5], rows[:, 6], rows, places[b].shapes))
-        return idx, out
+        if c[B] > cap or c[B] < 0 or any(k < 0 for k in c[:B]):  # rare: more candidates than the optimistic capacity -> re-run, blocking
+            torch.cuda.synchronize(self.device)   # the slots' plans are shared with batches in flight: drain them first
+            src, aux = pack(item, None)           # (its own pinned buffer: the batch's may hold a later, unlaunched one)
+            rec, pad_gain = detect(src.to(self.device), aux, 0)
+            packed, c = non_max_suppression_obb(rec, return_packed=True, **self.kw)
+            if pad_gain is not None:
+                hpoly = lb.scale_polys_batched(packed, torch.tensor(c, dtype=torch.int64).to(self.device), pad_gain).cpu()
+            hout = packed.cpu()
+        return emit(item, hout, hpoly, c[:B])

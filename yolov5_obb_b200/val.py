@@ -285,12 +285,8 @@ class Validator:
         if isinstance(x, torch.Tensor):
             return self.model.detect_records(x, augment=self.augment), tuple(x.shape)
         from . import letterbox as lb
-        from .general import DetectRecords
         buf, batch = x
-        shape = (batch.B, 3, batch.Hp, batch.Wp)
-        eng = self.model.records_plan(shape, self.device)
-        lb.letterbox_s2d(buf, batch, eng.x_s2d, 1)
-        return DetectRecords(eng.forward_s2d(), eng.nc, eng.half), shape
+        return lb.letterboxed_records(self.model, buf, batch, self.device)[0], (batch.B, 3, batch.Hp, batch.Wp)
 
     def __call__(self, batches) -> ValMetrics:
         nc = self.model.nc if hasattr(self.model, "nc") else self.model.model[-1].nc   # (an Ensemble has `nc`)
