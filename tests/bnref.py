@@ -35,6 +35,13 @@ def stat_blocks(npix: int, C: int, sms: int) -> int:
     return max(1, min(want, 4 * sms))
 
 
+def colwise_grid(npix: int, C: int, sms: int):
+    """colwise_grid() of k_bn_silu_apply / k_bn_bwd_apply: (x blocks, y column groups).  A block steps over 2 * lanes pixels
+    (two per thread), at most 8 blocks per SM; a y block per group of `cols` vector columns."""
+    vecs, cols, lanes = stat_layout(C)
+    return max(1, min(-(-npix // (2 * lanes)), 8 * sms)), -(-vecs // cols)
+
+
 def stat_geometry(npix: int, C: int, sms: int):
     """(blocks, chunk, lanes) of one statistics launch."""
     blocks = stat_blocks(npix, C, sms)

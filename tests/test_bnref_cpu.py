@@ -16,6 +16,10 @@ def test_geometry_of_the_benchmarked_stem_layer():
     assert bnref.stat_layout(2056) == (257, 256, 1)       # the second column group
     assert bnref.stat_layout(8) == (1, 1, 256)
     assert bnref.stat_blocks(2, 48, 132) == 1
+    # the element-wise kernels: 84 pixels per block step, capped at 8 blocks per SM; 2056 channels take two column groups
+    assert bnref.colwise_grid(8 * 512 * 512, 48, 132) == (1056, 1)
+    assert bnref.colwise_grid(85, 48, 132) == (2, 1)
+    assert bnref.colwise_grid(3, 2056, 132) == (2, 2)
 
 
 @pytest.mark.parametrize("npix,C,sms", [(2, 8, 4), (41, 48, 4), (42 * 16 * 16 + 1, 48, 4), (300, 16, 2), (255, 8, 1),

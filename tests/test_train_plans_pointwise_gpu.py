@@ -15,7 +15,9 @@ outside the op's write mask, and the reduction scratch is filled with NaN before
      plan with the arguments TrainEngine._forward_eager passes, and every non-conv step of their BackwardPlan alone through
      its own closure;
   3. the accumulate flags of the backward plan: each layer output's gradient range gets one overwrite, then one accumulate
-     per further consumer, counted from the model graph.
+     per further consumer, counted from the model graph (a layer whose gradient a frozen backbone prunes gets none).
+Section 2's checks take any train plan: a frozen backbone (train.py --freeze) and a plan carved from a multi-scale run's
+arena; tests/test_train_plans_pointwise_wide_gpu.py runs them on the P6, multi-scale and frozen plans.
 Worst error-to-bound ratios per launch kind are printed at the end of the module (run with -s)."""
 import inspect
 import time
@@ -27,9 +29,10 @@ from tests import bnref
 from tests.bnref import U, gamma, stat_chain, ulp32
 from tests.modelgen import build_mirror
 from yolov5_obb_b200 import _lib
-from yolov5_obb_b200.layout import _is, sources
+from yolov5_obb_b200.layout import _is, grad_liveness, shapes, sources
 from yolov5_obb_b200.train_backward import BackwardPlan
 from yolov5_obb_b200.train_engine import TrainEngine, _PoolLayer
+from yolov5_obb_b200.train_step import freeze_layers
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -294,8 +297,11 @@ def test_bn_stats_full_layer(ratio):
 APPLY_SHAPES = [(2, 5, 7, 48), (1, 3, 3, 2056), (2, 16, 24, 384), (1, 1, 1, 8), (3, 9, 11, 96)]
 
 
+APPLY_FLAGS = [(a, r, u) for a in (0, 1) for r in (0, 1) for u in (0, 1)]
+
+
 @pytest.mark.parametrize("shape", APPLY_SHAPES)
-@pytest.mark.parametrize("act,res,up", [(a, r, u) for a in (0, 1) for r in (0, 1) for u in (0, 1)])
+@pytest.mark.parametrize("act,res,up", APPLY_FLAGS)
 def test_bn_silu_apply(shape, act, res, up):
     B, H, W, C = shape
     g = torch.Generator(device=DEV).manual_seed(B * H * W + C)
@@ -369,7 +375,10 @@ def test_bn_silu_bwd(C, which, ratio, act, gmode, pacc):
               (dg, db, odg, odb, pacc), "bn_silu_bwd")
 
 
-@pytest.mark.parametrize("B,H,W,C", [(2, 5, 7, 16), (1, 1, 1, 8), (2, 8, 12, 2056), (3, 4, 3, 96)])
+UPSAMPLE_SHAPES = [(2, 5, 7, 16), (1, 1, 1, 8), (2, 8, 12, 2056), (3, 4, 3, 96)]
+
+
+@pytest.mark.parametrize("B,H,W,C", UPSAMPLE_SHAPES)
 @pytest.mark.parametrize("acc", [0, 1])
 def test_upsample2x_bwd(B, H, W, C, acc):
     g = torch.Generator(device=DEV).manual_seed(B + H + W + C)
@@ -389,7 +398,10 @@ def test_upsample2x_bwd(B, H, W, C, acc):
     note("upsample2x_bwd (bitwise)", 0.0)
 
 
-@pytest.mark.parametrize("npix,C,stride,c_off", [(37, 24, 40, 8), (5, 13, 16, 3), (4096, 96, 128, 16), (1, 8, 8, 0)])
+ADD_CASES = [(37, 24, 40, 8), (5, 13, 16, 3), (4096, 96, 128, 16), (1, 8, 8, 0)]
+
+
+@pytest.mark.parametrize("npix,C,stride,c_off", ADD_CASES)
 @pytest.mark.parametrize("acc", [0, 1])
 def test_add_f32_to_bf16(npix, C, stride, c_off, acc):
     g = torch.Generator(device=DEV).manual_seed(npix + C)
@@ -407,8 +419,10 @@ def test_add_f32_to_bf16(npix, C, stride, c_off, acc):
     note("add_f32_to_bf16 (bitwise)", 0.0)
 
 
-@pytest.mark.parametrize("B,na,H,W,no,bn", [(2, 3, 5, 7, 200, 208), (1, 3, 4, 4, 21, 24), (2, 2, 3, 5, 20, 24),
-                                            (1, 3, 1, 1, 7, 7)])
+PACK_SHAPES = [(2, 3, 5, 7, 200, 208), (1, 3, 4, 4, 21, 24), (2, 2, 3, 5, 20, 24), (1, 3, 1, 1, 7, 7)]
+
+
+@pytest.mark.parametrize("B,na,H,W,no,bn", PACK_SHAPES)
 def test_detect_grad_pack(B, na, H, W, no, bn):
     """The vec4 path (no, bn multiples of 4) and the one-channel path (odd no); padding channels written as 0."""
     gsrc = torch.Generator(device=DEV).manual_seed(no)
@@ -425,8 +439,11 @@ def test_detect_grad_pack(B, na, H, W, no, bn):
 POOL_SHAPES = [(2, 7, 9, 24), (1, 3, 4, 16), (1, 1, 1, 8), (2, 5, 5, 40), (1, 2, 11, 8), (2, 13, 6, 136)]
 
 
+POOL_FORMS = ["f32", "bf16", "f32+bf16"]
+
+
 @pytest.mark.parametrize("B,H,W,C", POOL_SHAPES)
-@pytest.mark.parametrize("form", ["f32", "bf16", "f32+bf16"])
+@pytest.mark.parametrize("form", POOL_FORMS)
 def test_maxpool5_bwd(B, H, W, C, form):
     """Small-integer activations (ties everywhere), dyadic gradients (fp32 atomics exact in any order): bit for bit against
     ATen's first-maximum routing, added onto what the fp32 buffer held."""
@@ -467,9 +484,19 @@ class _Recorder:
         return rec
 
 
-def _plan(size, B, H, W):
+def _plan(size, B, H, W, freeze=None, arena_hw=None):
+    """The yolov5{size} train plan at B x H x W.  freeze: train.py --freeze (freeze_layers; the backward plan is then built
+    for the requires_grad flags it leaves); arena_hw: carve the plan from an arena reserved for B x arena_hw, as train.py
+    --multi-scale does."""
     m = build_mirror(size, nc=15, seed=0).train().to(DEV)
-    return m, TrainEngine(m, B, H, W, DEV)
+    if freeze is not None:
+        freeze_layers(m, [freeze] if isinstance(freeze, int) else list(freeze))
+    arena = m.reserve_train_arena(B, *arena_hw, DEV) if arena_hw is not None else None
+    return m, TrainEngine(m, B, H, W, DEV, arena=arena)
+
+
+def _trainable(m):
+    return tuple(p.requires_grad for p in m.parameters())
 
 
 def _randomise_bn(m, g):
@@ -484,10 +511,15 @@ def _randomise_bn(m, g):
 
 
 @pytest.mark.parametrize("size,B,H,W", PLANS)
-def test_plan_forward_bn_launches(size, B, H, W):
+def test_plan_forward_bn_launches(size, B, H, W, freeze=None, arena_hw=None):
+    plan_forward_bn_launches(size, B, H, W, freeze, arena_hw)
+
+
+def plan_forward_bn_launches(size, B, H, W, freeze=None, arena_hw=None):
     """Every bn_batch_stats / bn_silu_apply pair of the train plan, issued with the arguments _forward_eager passes, on
-    controlled z (|mean| / sigma cycling through 0, 3, 10) with every other element of the destination buffers a sentinel."""
-    m, eng = _plan(size, B, H, W)
+    controlled z (|mean| / sigma cycling through 0, 3, 10) with every other element of the destination buffers a sentinel.
+    -> the number of BatchNorm layers."""
+    m, eng = _plan(size, B, H, W, freeze, arena_hw)
     g = torch.Generator(device=DEV).manual_seed(5)
     _randomise_bn(m, g)
     real = eng._L
@@ -545,23 +577,31 @@ def test_plan_forward_bn_launches(size, B, H, W):
     print(f"\n{size} b{B} {H}x{W}: {len(lays)} BatchNorm layers' forward launches checked ({n_res} with a residual, "
           f"{n_y2x} with a 2x copy)")
     assert n_y2x > 0 and n_res > 0
+    return len(lays)
 
 
 def _defaults(fn):
     return {k: p.default for k, p in inspect.signature(fn).parameters.items() if p.default is not inspect.Parameter.empty}
 
 
-def _consumers(m):
+def _consumers(m, H, W):
     """id(Conv module) -> how many gradient contributions its output receives, from the model graph: a top-level output
     gets one per consuming Conv / SPPF / Upsample / Detect, two per C3 (cv1 and cv2 both read it), and what its Concat gets;
-    inside a C3 / SPPF the counts follow the block's structure."""
+    inside a C3 / SPPF the counts follow the block's structure.  A consumer counts only where the plan produces its data
+    gradient: into the output of a layer whose gradient is needed (layout.grad_liveness under the model's requires_grad
+    flags; a frozen module's parameters all freeze together, so its inner convs share its liveness).  Every other output
+    gets none."""
     mods = list(m.model)
+    ch, _ = shapes(mods, H, W)
+    live, _ = grad_liveness(mods, ch, lambda mm: any(p.requires_grad for p in mm.parameters()))
     users = {}
     for mm in mods:
         for s in sources(mm):
             users.setdefault(s, []).append(mm)
 
     def E(i):
+        if i not in live:
+            return 0
         n = 0
         for mm in users.get(i, []):
             n += E(mm.i) if _is(mm, "Concat") else (2 if _is(mm, "C3") else 1)
@@ -569,27 +609,33 @@ def _consumers(m):
 
     cnt = {}
     for mm in mods:
+        on = int(mm.i in live)
         if _is(mm, "Conv"):
             cnt[id(mm)] = E(mm.i)
         elif _is(mm, "C3"):
             cnt[id(mm.cv3)] = E(mm.i)
-            cnt[id(mm.cv1)] = 1 + int(mm.m[0].add)
-            cnt[id(mm.cv2)] = 1
+            cnt[id(mm.cv1)] = on * (1 + int(mm.m[0].add))
+            cnt[id(mm.cv2)] = on
             for j, bt in enumerate(mm.m):
-                cnt[id(bt.cv1)] = 1
-                cnt[id(bt.cv2)] = 1 + int(mm.m[j + 1].add) if j + 1 < len(mm.m) else 1
+                cnt[id(bt.cv1)] = on
+                cnt[id(bt.cv2)] = on * (1 + int(mm.m[j + 1].add) if j + 1 < len(mm.m) else on)
         elif _is(mm, "SPPF"):
             cnt[id(mm.cv2)] = E(mm.i)
-            cnt[id(mm.cv1)] = 2        # cv2's data gradient of the whole concat, then the pool chain's add
+            cnt[id(mm.cv1)] = 2 * on   # cv2's data gradient of the whole concat, then the pool chain's add
     return cnt
 
 
 @pytest.mark.parametrize("size,B,H,W", PLANS)
-def test_plan_backward_steps(size, B, H, W):
+def test_plan_backward_steps(size, B, H, W, freeze=None, arena_hw=None):
+    plan_backward_steps(size, B, H, W, freeze, arena_hw)
+
+
+def plan_backward_steps(size, B, H, W, freeze=None, arena_hw=None):
     """Every non-conv step of BackwardPlan.steps alone through its own closure on sentinel-filled buffers, against section
-    1's references; then the accumulate flags of every gradient range in step order."""
-    m, eng = _plan(size, B, H, W)
-    plan = BackwardPlan(eng)
+    1's references; then the accumulate flags of every gradient range in step order.  -> (step kinds, the number of
+    gradient ranges whose flags were checked)."""
+    m, eng = _plan(size, B, H, W, freeze, arena_hw)
+    plan = BackwardPlan(eng, _trainable(m))
     g = torch.Generator(device=DEV).manual_seed(9)
     _randomise_bn(m, g)
     L, st = lib(), stream()
@@ -691,7 +737,9 @@ def test_plan_backward_steps(size, B, H, W):
                       (dg, db, torch.zeros_like(dg), torch.zeros_like(db), 0), kind)   # the plan overwrites dgamma / dbeta
         else:
             raise AssertionError(f"unexpected backward step {tag}")
-    need = {"detect_pack", "detect_bias", "upsample_bwd", "bn_bwd", "pool_bwd"}
+    need = {"detect_pack", "detect_bias", "upsample_bwd", "bn_bwd"}
+    if any(isinstance(lay, _PoolLayer) and i in plan._live_out for i, lay in enumerate(eng.layers)):
+        need.add("pool_bwd")      # (a frozen backbone takes SPPF's backward with it)
     assert need <= set(kinds), kinds
     print(f"\n{size} b{B} {H}x{W}: backward steps checked {kinds}")
 
@@ -718,9 +766,16 @@ def test_plan_backward_steps(size, B, H, W):
             contrib.append((r.buf.data_ptr(), r.c_off, r.C, int(a["gacc"]), "bn_bwd residual"))
         elif tag == "pool_bwd":
             contrib.append((a["gbase"], 0, a["c_"], 1, "pool add"))
-    cnt = _consumers(m)
+    cnt = _consumers(m, H, W)
     n_checked = 0
     for lay in eng.conv_layers:
+        if cnt[id(lay.mod)] == 0:   # pruned: nothing may write its gradient range (if its buffer has a gradient at all)
+            gb = plan.gbuf.get(lay.y.buf.data_ptr())
+            if gb is not None:
+                lo, hi = lay.y.c_off, lay.y.c_off + lay.y.C
+                hit = [c for c in contrib if c[0] == gb.data_ptr() and c[1] < hi and lo < c[1] + c[2]]
+                assert not hit, f"a pruned {type(lay.mod).__name__} output [{lo}, {hi}) receives gradient: {hit}"
+            continue
         gy = plan.gbuf[lay.y.buf.data_ptr()].data_ptr(), lay.y.c_off, lay.y.C
         seq = [(c[3], c[4]) for c in contrib if c[0] == gy[0] and c[1] <= gy[1] and gy[1] + gy[2] <= c[1] + c[2]]
         part = [c for c in contrib if c[0] == gy[0] and c[1] < gy[1] + gy[2] and gy[1] < c[1] + c[2]
@@ -731,3 +786,4 @@ def test_plan_backward_steps(size, B, H, W):
                                             f"flags {seq}, want {want}"
         n_checked += 1
     print(f"accumulate flags of {n_checked} gradient ranges match the model graph's consumer counts")
+    return kinds, n_checked
