@@ -331,6 +331,28 @@ int y5obb_bn_silu_bwd(const void* z, int64_t z_pix_stride, const void* dy, int64
                       float* sum_du, float* sum_dux, void* dz, int64_t dz_pix_stride, void* gres,
                       int64_t gres_pix_stride, int gres_accumulate, float* dgamma, float* dbeta, int param_accumulate,
                       float* scratch, int64_t scratch_floats, void* stream);
+
+/* SyncBatchNorm (torch.nn.SyncBatchNorm): y5obb_bn_batch_stats and y5obb_bn_silu_bwd split where the ranks all-reduce
+ * (SUM) a per-layer fp64 record.  A record summed over one rank gives bit for bit what the plain entry points give.
+ *   y5obb_bn_stats_sync            the rank's forward record rec[2C + 1] = [sum z (C) | sum z^2 (C) | npix]
+ *   y5obb_bn_finalize_sync         y5obb_bn_finalize from the summed record (global mean, var and count)
+ *   y5obb_bn_silu_bwd_reduce_sync  the rank's backward record rec[2C] = [sum du (C) | sum du * xhat (C)]; dgamma / dbeta
+ *                                  are the rank's own (a data-parallel gradient all-reduce sums them)
+ *   y5obb_bn_silu_bwd_apply_sync   dz over the npix local pixels from the summed backward record, with N = *n_all, the
+ *                                  summed forward record's count (rec_fwd + 2C) */
+int y5obb_bn_stats_sync(const void* z, int64_t z_pix_stride, int64_t npix, int C, double* rec, float* scratch,
+                        int64_t scratch_floats, void* stream);
+int y5obb_bn_finalize_sync(const double* rec, int C, const float* gamma, const float* beta, float eps, float momentum,
+                           float* running_mean, float* running_var, float* scale, float* shift, float* mean_out,
+                           float* invstd_out, void* stream);
+int y5obb_bn_silu_bwd_reduce_sync(const void* z, int64_t z_pix_stride, const void* dy, int64_t dy_pix_stride, int64_t npix,
+                                  int C, const float* scale, const float* shift, const float* mean, const float* invstd,
+                                  int act, double* rec, float* dgamma, float* dbeta, int param_accumulate, float* scratch,
+                                  int64_t scratch_floats, void* stream);
+int y5obb_bn_silu_bwd_apply_sync(const void* z, int64_t z_pix_stride, const void* dy, int64_t dy_pix_stride, int64_t npix,
+                                 int C, const float* scale, const float* shift, const float* mean, const float* invstd,
+                                 int act, const double* rec, const double* n_all, void* dz, int64_t dz_pix_stride,
+                                 void* gres, int64_t gres_pix_stride, int gres_accumulate, void* stream);
 /* ---- weight gradient (wgmma GEMM over the pixel axis) ---------------------------------------------
  * dW[tap][co][ci] (fp32, ACCUMULATED with atomics: zero it first) = sum_{b,ho,wo} dz[b,ho,wo,co] * x[b,s*ho+kh-ph,s*wo+kw-pw,ci].
  * Replaces the cuDNN wgrad autograd calls for models/common.py:37-46 under train.py:333.  Operands are the NHWC bf16

@@ -64,6 +64,15 @@ PROTOTYPES = {
     "y5obb_bn_silu_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_int,
                                   c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p]),
+    "y5obb_bn_stats_sync": (c_int, [c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
+    "y5obb_bn_finalize_sync": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p]),
+    "y5obb_bn_silu_bwd_reduce_sync": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p,
+                                              c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                              c_int64, c_void_p]),
+    "y5obb_bn_silu_bwd_apply_sync": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                             c_int64, c_int, c_void_p]),
     "y5obb_wgrad_create": (c_int, [c_void_p, ctypes.POINTER(c_void_p)]),
     "y5obb_wgrad_run": (c_int, [c_void_p, c_void_p]),
     "y5obb_wgrad_schedule": (c_int, [c_void_p] + [ctypes.POINTER(c_int)] * 14),

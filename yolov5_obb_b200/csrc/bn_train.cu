@@ -14,6 +14,7 @@
 #include <cuda_bf16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -138,10 +139,11 @@ __global__ void __launch_bounds__(STAT_THREADS) k_bn_stats(const __nv_bfloat16* 
 // out[j] = sum over blocks of partial[b][j], j in [0, 2C): [0, C) -> out_a, [C, 2C) -> out_b, in a FIXED order: thread
 // (seg, col) adds rows seg, seg + 32, ... and thread (0, col) then adds the 32 segment sums.  8 columns x 32 row
 // segments per block.  Optionally also writes the BatchNorm parameter gradients dgamma (+)= out_b, dbeta (+)= out_a.
-__global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict__ partial, int blocks, int C,
-                                                         float* __restrict__ out_a, float* __restrict__ out_b,
-                                                         float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                                         int param_accumulate) {
+// T = double: the fp32 sums are widened once, into a SyncBatchNorm record (k_reduce_partials_rec).
+template <typename T>
+__device__ __forceinline__ void reduce_partials(const float* __restrict__ partial, int blocks, int C, T* __restrict__ out_a,
+                                                T* __restrict__ out_b, float* __restrict__ dgamma,
+                                                float* __restrict__ dbeta, int param_accumulate) {
   __shared__ float red[32][8];
   const int col = threadIdx.x & 7, seg = threadIdx.x >> 3;
   const int j = blockIdx.x * 8 + col;
@@ -164,14 +166,32 @@ __global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict
   }
 }
 
+__global__ void __launch_bounds__(256) k_reduce_partials(const float* __restrict__ partial, int blocks, int C,
+                                                         float* __restrict__ out_a, float* __restrict__ out_b,
+                                                         float* __restrict__ dgamma, float* __restrict__ dbeta,
+                                                         int param_accumulate) {
+  reduce_partials(partial, blocks, C, out_a, out_b, dgamma, dbeta, param_accumulate);
+}
+
+// SyncBatchNorm backward, first half: the rank's record [sum(du) (C) | sum(du * xhat) (C)] in fp64, local dgamma / dbeta
+__global__ void __launch_bounds__(256) k_reduce_partials_rec(const float* __restrict__ partial, int blocks, int C,
+                                                             double* __restrict__ rec, float* __restrict__ dgamma,
+                                                             float* __restrict__ dbeta, int param_accumulate) {
+  reduce_partials(partial, blocks, C, rec, rec + C, dgamma, dbeta, param_accumulate);
+}
+
 // k_reduce_partials + k_bn_finalize in one launch: thread (seg, col) adds rows seg, seg + 32, ... of BOTH statistics of
 // channel c, thread (0, col) adds the 32 segment sums in order and finalises the channel.
-__global__ void __launch_bounds__(256) k_reduce_finalize(const float* __restrict__ partial, int blocks, long long npix, int C,
-                                                         const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                         float eps, float momentum, float* __restrict__ running_mean,
-                                                         float* __restrict__ running_var, float* __restrict__ scale,
-                                                         float* __restrict__ shift, float* __restrict__ mean_out,
-                                                         float* __restrict__ invstd_out) {
+// RECORD (k_reduce_stats_rec): the thread stores the sums instead, as the rank's SyncBatchNorm record
+// rec[2C + 1] = [sum (C) | sum of squares (C) | n] in fp64 (the fp32 sums widened once; an fp32 count would be inexact
+// above 2^24 pixels), which k_bn_finalize_rec finalises once every rank's record is added in.
+template <bool RECORD>
+__device__ __forceinline__ void reduce_finalize(const float* __restrict__ partial, int blocks, long long npix, int C,
+                                                const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                                                float momentum, float* __restrict__ running_mean,
+                                                float* __restrict__ running_var, float* __restrict__ scale,
+                                                float* __restrict__ shift, float* __restrict__ mean_out,
+                                                float* __restrict__ invstd_out, double* __restrict__ rec) {
   __shared__ float red[2][32][8];
   const int col = threadIdx.x & 7, seg = threadIdx.x >> 3;
   const int c = blockIdx.x * 8 + col;
@@ -191,9 +211,63 @@ __global__ void __launch_bounds__(256) k_reduce_finalize(const float* __restrict
     sum += red[0][s2][col];
     sumsq += red[1][s2][col];
   }
+  if (RECORD) {
+    rec[c] = (double)sum;
+    rec[C + c] = (double)sumsq;
+    if (c == 0) rec[2 * C] = (double)npix;
+    return;
+  }
   const double n = (double)npix;
   const double m = (double)sum / n;
   double var = (double)sumsq / n - m * m;
+  if (var < 0) var = 0;
+  const float invstd = (float)(1.0 / sqrt(var + (double)eps));
+  const float sc = gamma[c] * invstd;
+  scale[c] = sc;
+  shift[c] = beta[c] - (float)m * sc;
+  mean_out[c] = (float)m;
+  invstd_out[c] = invstd;
+  if (running_mean) {
+    const double unbiased = n > 1 ? var * n / (n - 1.0) : var;
+    running_mean[c] = (1.0f - momentum) * running_mean[c] + momentum * (float)m;
+    running_var[c] = (1.0f - momentum) * running_var[c] + momentum * (float)unbiased;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_reduce_finalize(const float* __restrict__ partial, int blocks, long long npix, int C,
+                                                         const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                         float eps, float momentum, float* __restrict__ running_mean,
+                                                         float* __restrict__ running_var, float* __restrict__ scale,
+                                                         float* __restrict__ shift, float* __restrict__ mean_out,
+                                                         float* __restrict__ invstd_out) {
+  reduce_finalize<false>(partial, blocks, npix, C, gamma, beta, eps, momentum, running_mean, running_var, scale, shift,
+                         mean_out, invstd_out, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_reduce_stats_rec(const float* __restrict__ partial, int blocks, long long npix, int C,
+                                                          double* __restrict__ rec) {
+  reduce_finalize<true>(partial, blocks, npix, C, nullptr, nullptr, 0.f, 0.f, nullptr, nullptr, nullptr, nullptr, nullptr,
+                        nullptr, rec);
+}
+
+// mean, biased var -> invstd, scale, shift; running statistics with the unbiased var over n pixels (torch.nn.BatchNorm2d).
+// S = double (k_bn_finalize_rec): sums and count from a SyncBatchNorm record added over every rank.
+template <typename S>
+__device__ __forceinline__ void bn_finalize(const S* __restrict__ sum, const S* __restrict__ sumsq, long long npix,
+                                            const double* __restrict__ n_all, int C, const float* __restrict__ gamma,
+                                            const float* __restrict__ beta, float eps, float momentum,
+                                            float* __restrict__ running_mean, float* __restrict__ running_var,
+                                            float* __restrict__ scale, float* __restrict__ shift,
+                                            float* __restrict__ mean_out, float* __restrict__ invstd_out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  double n;
+  if constexpr (std::is_same<S, double>::value)
+    n = *n_all;
+  else
+    n = (double)npix;
+  const double m = (double)sum[c] / n;
+  double var = (double)sumsq[c] / n - m * m;
   if (var < 0) var = 0;
   const float invstd = (float)(1.0 / sqrt(var + (double)eps));
   const float sc = gamma[c] * invstd;
@@ -213,23 +287,17 @@ __global__ void k_bn_finalize(const float* __restrict__ sum, const float* __rest
                               float* __restrict__ running_mean, float* __restrict__ running_var,
                               float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ mean_out,
                               float* __restrict__ invstd_out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const double n = (double)npix;
-  const double m = (double)sum[c] / n;
-  double var = (double)sumsq[c] / n - m * m;
-  if (var < 0) var = 0;
-  const float invstd = (float)(1.0 / sqrt(var + (double)eps));
-  const float sc = gamma[c] * invstd;
-  scale[c] = sc;
-  shift[c] = beta[c] - (float)m * sc;
-  mean_out[c] = (float)m;
-  invstd_out[c] = invstd;
-  if (running_mean) {
-    const double unbiased = n > 1 ? var * n / (n - 1.0) : var;
-    running_mean[c] = (1.0f - momentum) * running_mean[c] + momentum * (float)m;
-    running_var[c] = (1.0f - momentum) * running_var[c] + momentum * (float)unbiased;
-  }
+  bn_finalize(sum, sumsq, npix, nullptr, C, gamma, beta, eps, momentum, running_mean, running_var, scale, shift, mean_out,
+              invstd_out);
+}
+
+// SyncBatchNorm forward, second half: rec = the records of every rank added up (its sums and its count rec[2C])
+__global__ void k_bn_finalize_rec(const double* __restrict__ rec, int C, const float* __restrict__ gamma,
+                                  const float* __restrict__ beta, float eps, float momentum, float* __restrict__ running_mean,
+                                  float* __restrict__ running_var, float* __restrict__ scale, float* __restrict__ shift,
+                                  float* __restrict__ mean_out, float* __restrict__ invstd_out) {
+  bn_finalize(rec, rec + C, 0, rec + 2 * C, C, gamma, beta, eps, momentum, running_mean, running_var, scale, shift, mean_out,
+              invstd_out);
 }
 
 // sigmoid through the hardware tanh (one MUFU op, |rel err| ~ 2^-11: far below the bf16 the results are stored in)
@@ -384,30 +452,37 @@ __global__ void __launch_bounds__(STAT_THREADS) k_bn_bwd_reduce(const __nv_bfloa
 // dz = scale * (du - sum_du / N - xhat * sum_dux / N) = k1 * du + k2 * z + k3 with per-channel k1 = scale,
 // k2 = -scale * invstd * sum_dux / N, k3 = scale * (mean * invstd * sum_dux / N - sum_du / N);
 // optional pass-through of dy into the residual branch.  Column-persistent threads (see k_bn_silu_apply).
-__global__ void __launch_bounds__(256) k_bn_bwd_apply(const __nv_bfloat16* __restrict__ z, long long z_stride,
-                                                      const __nv_bfloat16* __restrict__ dy, long long dy_stride, long long npix,
-                                                      int C, const float* __restrict__ scale, const float* __restrict__ shift,
-                                                      const float* __restrict__ mean, const float* __restrict__ invstd, int act,
-                                                      const float* __restrict__ sum_du, const float* __restrict__ sum_dux,
-                                                      __nv_bfloat16* __restrict__ dz, long long dz_stride,
-                                                      __nv_bfloat16* __restrict__ gres, long long gres_stride,
-                                                      int gres_accumulate) {
+// S = double (k_bn_bwd_apply_rec): the sums come from a SyncBatchNorm record summed over every rank and N is the forward
+// record's count `n_all`; the loop still covers the npix local pixels.
+template <typename S>
+__device__ __forceinline__ void bn_bwd_apply(const __nv_bfloat16* __restrict__ z, long long z_stride,
+                                             const __nv_bfloat16* __restrict__ dy, long long dy_stride, long long npix, int C,
+                                             const float* __restrict__ scale, const float* __restrict__ shift,
+                                             const float* __restrict__ mean, const float* __restrict__ invstd, int act,
+                                             const S* __restrict__ sum_du, const S* __restrict__ sum_dux,
+                                             const double* __restrict__ n_all, __nv_bfloat16* __restrict__ dz,
+                                             long long dz_stride, __nv_bfloat16* __restrict__ gres, long long gres_stride,
+                                             int gres_accumulate) {
   const int vecs = C >> 3;
   const int cols = min(vecs, 256);
   const int lanes = 256 / cols;
   const int col_in = threadIdx.x % cols, lane = threadIdx.x / cols;
   const int cv = blockIdx.y * cols + col_in;
   if (cv >= vecs || lane >= lanes) return;
-  const float inv_n = 1.0f / (float)npix;
+  float inv_n;
+  if constexpr (std::is_same<S, double>::value)
+    inv_n = 1.0f / (float)*n_all;
+  else
+    inv_n = 1.0f / (float)npix;
   float sc[8], sh[8], k2[8], k3[8];
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const int c = cv * 8 + k;
     sc[k] = scale[c];
     sh[k] = shift[c];
-    const float b = invstd[c] * sum_dux[c] * inv_n;
+    const float b = invstd[c] * (float)sum_dux[c] * inv_n;
     k2[k] = -sc[k] * b;
-    k3[k] = sc[k] * (mean[c] * b - sum_du[c] * inv_n);
+    k3[k] = sc[k] * (mean[c] * b - (float)sum_du[c] * inv_n);
   }
   const long long step = (long long)gridDim.x * lanes;
   for (long long p = (long long)blockIdx.x * lanes + lane; p < npix; p += 2 * step) {
@@ -452,6 +527,33 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply(const __nv_bfloat16* __res
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(256) k_bn_bwd_apply(const __nv_bfloat16* __restrict__ z, long long z_stride,
+                                                      const __nv_bfloat16* __restrict__ dy, long long dy_stride, long long npix,
+                                                      int C, const float* __restrict__ scale, const float* __restrict__ shift,
+                                                      const float* __restrict__ mean, const float* __restrict__ invstd, int act,
+                                                      const float* __restrict__ sum_du, const float* __restrict__ sum_dux,
+                                                      __nv_bfloat16* __restrict__ dz, long long dz_stride,
+                                                      __nv_bfloat16* __restrict__ gres, long long gres_stride,
+                                                      int gres_accumulate) {
+  bn_bwd_apply(z, z_stride, dy, dy_stride, npix, C, scale, shift, mean, invstd, act, sum_du, sum_dux, nullptr, dz, dz_stride,
+               gres, gres_stride, gres_accumulate);
+}
+
+// SyncBatchNorm backward, second half: rec = [sum(du) | sum(du * xhat)] summed over every rank, n_all = the summed forward
+// record's count
+__global__ void __launch_bounds__(256) k_bn_bwd_apply_rec(const __nv_bfloat16* __restrict__ z, long long z_stride,
+                                                          const __nv_bfloat16* __restrict__ dy, long long dy_stride,
+                                                          long long npix, int C, const float* __restrict__ scale,
+                                                          const float* __restrict__ shift, const float* __restrict__ mean,
+                                                          const float* __restrict__ invstd, int act,
+                                                          const double* __restrict__ rec, const double* __restrict__ n_all,
+                                                          __nv_bfloat16* __restrict__ dz, long long dz_stride,
+                                                          __nv_bfloat16* __restrict__ gres, long long gres_stride,
+                                                          int gres_accumulate) {
+  bn_bwd_apply(z, z_stride, dy, dy_stride, npix, C, scale, shift, mean, invstd, act, rec, rec + C, n_all, dz, dz_stride, gres,
+               gres_stride, gres_accumulate);
 }
 
 // gdst[b,h,w,:] (+)= sum of the 2x2 block gsrc[b,2h+{0,1},2w+{0,1},:]   (backward of nn.Upsample(2x nearest))
@@ -701,6 +803,74 @@ int y5obb_bn_silu_bwd(const void* z, int64_t z_pix_stride, const void* dy, int64
                                      static_cast<const __nv_bfloat16*>(dy), dy_pix_stride, npix, C, scale, shift, mean,
                                      invstd, act, sum_du, sum_dux, static_cast<__nv_bfloat16*>(dz), dz_pix_stride,
                                      static_cast<__nv_bfloat16*>(gres), gres_pix_stride, gres_accumulate);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+int y5obb_bn_stats_sync(const void* z, int64_t z_pix_stride, int64_t npix, int C, double* rec, float* scratch,
+                        int64_t scratch_floats, void* stream) {
+  if (!z || !rec || !scratch || npix <= 0 || C <= 0 || (C & 7) || (z_pix_stride & 7)) return Y5OBB_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(scratch)) & 15) return Y5OBB_EINVAL;
+  const int blocks = stat_blocks(npix, C);
+  if (scratch_floats < (int64_t)blocks * 2 * C) return Y5OBB_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long chunk = (npix + blocks - 1) / blocks;
+  k_bn_stats<<<blocks, STAT_THREADS, 0, st>>>(static_cast<const __nv_bfloat16*>(z), z_pix_stride, npix, C, chunk, scratch);
+  Y5_LAUNCH_CHECK();
+  k_reduce_stats_rec<<<(C + 7) / 8, 256, 0, st>>>(scratch, blocks, npix, C, rec);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+int y5obb_bn_finalize_sync(const double* rec, int C, const float* gamma, const float* beta, float eps, float momentum,
+                           float* running_mean, float* running_var, float* scale, float* shift, float* mean_out,
+                           float* invstd_out, void* stream) {
+  if (!rec || !gamma || !beta || !scale || !shift || !mean_out || !invstd_out || C <= 0) return Y5OBB_EINVAL;
+  if ((running_mean == nullptr) != (running_var == nullptr)) return Y5OBB_EINVAL;
+  k_bn_finalize_rec<<<(C + 127) / 128, 128, 0, (cudaStream_t)stream>>>(rec, C, gamma, beta, eps, momentum, running_mean,
+                                                                        running_var, scale, shift, mean_out, invstd_out);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+int y5obb_bn_silu_bwd_reduce_sync(const void* z, int64_t z_pix_stride, const void* dy, int64_t dy_pix_stride, int64_t npix,
+                                  int C, const float* scale, const float* shift, const float* mean, const float* invstd,
+                                  int act, double* rec, float* dgamma, float* dbeta, int param_accumulate, float* scratch,
+                                  int64_t scratch_floats, void* stream) {
+  if ((dgamma == nullptr) != (dbeta == nullptr)) return Y5OBB_EINVAL;
+  if (!z || !dy || !scale || !shift || !mean || !invstd || !rec || !scratch || npix <= 0 || C <= 0 || (C & 7))
+    return Y5OBB_EINVAL;
+  if ((z_pix_stride & 7) || (dy_pix_stride & 7)) return Y5OBB_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(scratch)) & 15)
+    return Y5OBB_EINVAL;
+  const int blocks = stat_blocks(npix, C);
+  if (scratch_floats < (int64_t)blocks * 2 * C) return Y5OBB_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long chunk = (npix + blocks - 1) / blocks;
+  k_bn_bwd_reduce<<<blocks, STAT_THREADS, 0, st>>>(static_cast<const __nv_bfloat16*>(z), z_pix_stride,
+                                                   static_cast<const __nv_bfloat16*>(dy), dy_pix_stride, npix, C, scale,
+                                                   shift, mean, invstd, act, chunk, scratch);
+  Y5_LAUNCH_CHECK();
+  k_reduce_partials_rec<<<(2 * C + 7) / 8, 256, 0, st>>>(scratch, blocks, C, rec, dgamma, dbeta, param_accumulate);
+  Y5_LAUNCH_CHECK();
+  return Y5OBB_OK;
+}
+
+int y5obb_bn_silu_bwd_apply_sync(const void* z, int64_t z_pix_stride, const void* dy, int64_t dy_pix_stride, int64_t npix,
+                                 int C, const float* scale, const float* shift, const float* mean, const float* invstd,
+                                 int act, const double* rec, const double* n_all, void* dz, int64_t dz_pix_stride,
+                                 void* gres, int64_t gres_pix_stride, int gres_accumulate, void* stream) {
+  if (!z || !dy || !scale || !shift || !mean || !invstd || !rec || !n_all || !dz || npix <= 0 || C <= 0 || (C & 7))
+    return Y5OBB_EINVAL;
+  if ((z_pix_stride & 7) || (dy_pix_stride & 7) || (dz_pix_stride & 7) || (gres && (gres_pix_stride & 7))) return Y5OBB_EINVAL;
+  if ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dz) |
+       reinterpret_cast<uintptr_t>(gres)) & 15)
+    return Y5OBB_EINVAL;
+  const dim3 g2 = colwise_grid(npix, C);
+  k_bn_bwd_apply_rec<<<g2, 256, 0, (cudaStream_t)stream>>>(
+      static_cast<const __nv_bfloat16*>(z), z_pix_stride, static_cast<const __nv_bfloat16*>(dy), dy_pix_stride, npix, C, scale,
+      shift, mean, invstd, act, rec, n_all, static_cast<__nv_bfloat16*>(dz), dz_pix_stride, static_cast<__nv_bfloat16*>(gres),
+      gres_pix_stride, gres_accumulate);
   Y5_LAUNCH_CHECK();
   return Y5OBB_OK;
 }

@@ -196,6 +196,14 @@ class BackwardPlan:
                 self.keep.append(op)
 
         # ---------------- conv layers, reverse ----------------
+        # SyncBatchNorm (eng.bn_group): one fp64 record [sum du (C) | sum du * xhat (C)] per live BatchNorm backward, in one
+        # buffer outside the arena, all-reduced between its reduce and apply launches on the main chain
+        self.bn_rec = None
+        if eng.bn_group is not None:
+            n_rec = sum(2 * eng.layers[li].z.C for li in self._live_out if isinstance(li, int)
+                        and not isinstance(eng.layers[li], _PoolLayer))
+            self.bn_rec = torch.zeros(max(n_rec, 1), dtype=torch.float64, device=dev)
+        rec_off = 0
         self.conv_parts = []
         for li in reversed(range(len(eng.layers))):
             lay = eng.layers[li]
@@ -248,14 +256,34 @@ class BackwardPlan:
 
             dg, db = grad_of(bn.weight), grad_of(bn.bias)
 
-            def bn_bwd(st, lay=lay, z=z, gy=gy, dz=dz, s1=s1, s2=s2, gres=gres, gacc=gacc, npix=npix, C=Cout, dg=dg, db=db):
-                _lib.check(L.y5obb_bn_silu_bwd(z.ptr, z.pix_stride, gy.ptr, gy.pix_stride, npix, C, lay.scale.data_ptr(),
-                                               lay.shift.data_ptr(), lay.mean.data_ptr(), lay.invstd.data_ptr(), int(lay.act),
-                                               s1.data_ptr(), s2.data_ptr(), dz.data_ptr(), C,
-                                               gres.ptr if gres else None, gres.pix_stride if gres else 0, gacc,
-                                               dg.data_ptr(), db.data_ptr(), 0, eng.scratch.data_ptr(), eng.scratch.numel(), st),
-                           "bn_silu_bwd")
-            add("bn_bwd", bn_bwd)
+            if self.bn_rec is None:
+                def bn_bwd(st, lay=lay, z=z, gy=gy, dz=dz, s1=s1, s2=s2, gres=gres, gacc=gacc, npix=npix, C=Cout, dg=dg, db=db):
+                    _lib.check(L.y5obb_bn_silu_bwd(z.ptr, z.pix_stride, gy.ptr, gy.pix_stride, npix, C, lay.scale.data_ptr(),
+                                                   lay.shift.data_ptr(), lay.mean.data_ptr(), lay.invstd.data_ptr(),
+                                                   int(lay.act), s1.data_ptr(), s2.data_ptr(), dz.data_ptr(), C,
+                                                   gres.ptr if gres else None, gres.pix_stride if gres else 0, gacc,
+                                                   dg.data_ptr(), db.data_ptr(), 0, eng.scratch.data_ptr(), eng.scratch.numel(),
+                                                   st), "bn_silu_bwd")
+                add("bn_bwd", bn_bwd)
+            else:   # SyncBatchNorm: local sums -> SUM over the group -> dz with the global sums and count
+                rec = self.bn_rec[rec_off:rec_off + 2 * Cout]
+                rec_off += 2 * Cout
+
+                def bn_bwd_reduce(st, lay=lay, z=z, gy=gy, rec=rec, npix=npix, C=Cout, dg=dg, db=db):
+                    _lib.check(L.y5obb_bn_silu_bwd_reduce_sync(
+                        z.ptr, z.pix_stride, gy.ptr, gy.pix_stride, npix, C, lay.scale.data_ptr(), lay.shift.data_ptr(),
+                        lay.mean.data_ptr(), lay.invstd.data_ptr(), int(lay.act), rec.data_ptr(), dg.data_ptr(), db.data_ptr(),
+                        0, eng.scratch.data_ptr(), eng.scratch.numel(), st), "bn_silu_bwd_reduce_sync")
+
+                def bn_bwd_apply(st, lay=lay, z=z, gy=gy, dz=dz, rec=rec, gres=gres, gacc=gacc, npix=npix, C=Cout):
+                    _lib.check(L.y5obb_bn_silu_bwd_apply_sync(
+                        z.ptr, z.pix_stride, gy.ptr, gy.pix_stride, npix, C, lay.scale.data_ptr(), lay.shift.data_ptr(),
+                        lay.mean.data_ptr(), lay.invstd.data_ptr(), int(lay.act), rec.data_ptr(), lay.rec[2 * C:].data_ptr(),
+                        dz.data_ptr(), C, gres.ptr if gres else None, gres.pix_stride if gres else 0, gacc, st),
+                        "bn_silu_bwd_apply_sync")
+                add("bn_bwd_reduce", bn_bwd_reduce)
+                add("bn_allreduce", lambda st, rec=rec: eng._all_reduce(rec))
+                add("bn_bwd_apply", bn_bwd_apply)
 
             # ---- wgrad (straight from the NHWC buffers)
             x = lay.x

@@ -116,11 +116,16 @@ class _PoolLayer(NamedTuple):
 
 class TrainEngine:
     def __init__(self, model, B: int, H: int, W: int, device, in_hw=None, arena: Optional[TrainArena] = None,
-                 carver: Optional[_Carver] = None):
+                 carver: Optional[_Carver] = None, bn_group=None):
         """in_hw: (H_in, W_in) of the input when it differs from the planned (H, W): the plan's first launch is then the
         bilinear resize of train.py's --multi-scale (F.interpolate, align_corners=False) straight into the stem input.
         arena: carve every activation / gradient buffer from that TrainArena (Model.reserve_train_arena); carver: an
-        explicit allocator (the arena sizing pass)."""
+        explicit allocator (the arena sizing pass).
+        bn_group: a torch.distributed process group: every BatchNorm is a SyncBatchNorm over it (train.py --sync-bn,
+        torch.nn.SyncBatchNorm).  Each layer's batch statistics are all-reduced between the stats and finalize launches
+        (and its gradient sums in the backward plan), as one fp64 record [sum (C) | sum of squares (C) | pixel count] per
+        layer, so ranks may train at different sizes.  With an NCCL group the collectives are captured in the forward
+        and backward graphs; with any other backend (gloo) the plans run eagerly."""
         device = torch.device(device)
         if device.type != "cuda":
             raise RuntimeError("TrainEngine needs a CUDA device (sm_90a); there is no CPU path")
@@ -229,6 +234,18 @@ class TrainEngine:
         self.use_graph = os.environ.get("Y5OBB_NO_GRAPH", "0") != "1"
         self._graphs = {}
         self._nbt = [lay.mod.bn.num_batches_tracked for lay in self.conv_layers]
+        self.bn_group = bn_group
+        self.bn_rec = None
+        if bn_group is not None:
+            import torch.distributed as dist
+            if dist.get_backend(bn_group) != "nccl":   # (gloo's CUDA all_reduce cannot be captured)
+                self.use_graph = False
+            # every layer's SyncBatchNorm record [sum | sum of squares | n] in one fp64 buffer, outside the arena
+            self.bn_rec = torch.zeros(sum(2 * lay.z.C + 1 for lay in self.conv_layers), dtype=torch.float64, device=device)
+            o = 0
+            for lay in self.conv_layers:
+                lay.rec = self.bn_rec[o:o + 2 * lay.z.C + 1]
+                o += 2 * lay.z.C + 1
         cmax = max([lay.z.C for lay in self.conv_layers] + [det.na * 256])
         self.scratch = torch.zeros(int(L.y5obb_bn_scratch_floats(cmax)), dtype=torch.float32, device=device)  # reductions
         # device bytes this plan holds outside the arena (BatchNorm vectors, packed weights, scratch; later the backward
@@ -340,10 +357,20 @@ class TrainEngine:
                 z, y = lay.z, lay.y
                 npix = z.B * z.H * z.W
                 bn = lay.mod.bn
-                run("bn_stats", lambda: L.y5obb_bn_batch_stats(
-                    z.ptr, z.pix_stride, npix, z.C, bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps), float(bn.momentum),
-                    bn.running_mean.data_ptr(), bn.running_var.data_ptr(), lay.scale.data_ptr(), lay.shift.data_ptr(),
-                    lay.mean.data_ptr(), lay.invstd.data_ptr(), self.scratch.data_ptr(), self.scratch.numel(), st))
+                if self.bn_group is None:
+                    run("bn_stats", lambda: L.y5obb_bn_batch_stats(
+                        z.ptr, z.pix_stride, npix, z.C, bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps),
+                        float(bn.momentum), bn.running_mean.data_ptr(), bn.running_var.data_ptr(), lay.scale.data_ptr(),
+                        lay.shift.data_ptr(), lay.mean.data_ptr(), lay.invstd.data_ptr(), self.scratch.data_ptr(),
+                        self.scratch.numel(), st))
+                else:   # SyncBatchNorm: the rank's record, summed over the group, finalised with the global count
+                    run("bn_stats", lambda: L.y5obb_bn_stats_sync(z.ptr, z.pix_stride, npix, z.C, lay.rec.data_ptr(),
+                                                                  self.scratch.data_ptr(), self.scratch.numel(), st))
+                    self._all_reduce(lay.rec)
+                    run("bn_finalize", lambda: L.y5obb_bn_finalize_sync(
+                        lay.rec.data_ptr(), z.C, bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps), float(bn.momentum),
+                        bn.running_mean.data_ptr(), bn.running_var.data_ptr(), lay.scale.data_ptr(), lay.shift.data_ptr(),
+                        lay.mean.data_ptr(), lay.invstd.data_ptr(), st))
                 run("bn_apply", lambda: L.y5obb_bn_silu_apply(
                     z.ptr, z.pix_stride, npix, z.C, z.W, lay.scale.data_ptr(), lay.shift.data_ptr(), int(lay.act),
                     lay.res.ptr if lay.res else None, lay.res.pix_stride if lay.res else 0, y.ptr, y.pix_stride,
@@ -357,6 +384,11 @@ class TrainEngine:
             for tag, e0, e1 in evs:
                 self.prof.setdefault(tag, []).append(e0.elapsed_time(e1))
         return self.det_out
+
+    def _all_reduce(self, rec: torch.Tensor):
+        """SUM of a SyncBatchNorm record over bn_group, ordered on the current stream (captured with the graph under NCCL)."""
+        import torch.distributed as dist
+        dist.all_reduce(rec, op=dist.ReduceOp.SUM, group=self.bn_group)
 
     def backward(self, grads, trainable=None):
         """grads: dLoss/d(det_out[l]) for the three levels -> the BackwardPlan, whose .flat holds every parameter

@@ -128,7 +128,7 @@ class TrainStep:
 
     def __init__(self, model, hyp: Optional[dict] = None, batch_size: int = 16, imgsz: int = 1024, ema: bool = True,
                  warmup_iters: int = 0, multi_scale: bool = False, seed: Optional[int] = None, adam: bool = False,
-                 freeze=(0,)):
+                 freeze=(0,), sync_bn: bool = False):
         """warmup_iters > 0: the warm-up of train.py:305-316 over that many iterations (the reference uses
         max(round(warmup_epochs * batches_per_epoch), 1000)): every group's lr is interpolated from 0 (biases: from
         hyp['warmup_bias_lr']) to lr0 and the momentum from hyp['warmup_momentum'] to hyp['momentum'].
@@ -154,7 +154,13 @@ class TrainStep:
         only they would need.  requires_grad may also be changed between steps (unfreezing after some epochs): the next
         step builds the plan for the new flags.  With adam=True, once a frozen parameter becomes trainable torch.optim.Adam
         keeps a step count per parameter, which the fused kernel cannot follow: the step then uses torch.optim.Adam and
-        the foreach EMA for the rest of the run."""
+        the foreach EMA for the rest of the run.
+
+        sync_bn=True: train.py --sync-bn (torch.nn.SyncBatchNorm.convert_sync_batchnorm, train.py:207-210).  In an
+        initialised process group of more than one rank, every BatchNorm of the training plans uses the batch statistics
+        of all ranks (the default group: model.bn_group), its per-layer sums and pixel counts all-reduced inside the
+        forward plan and its gradient sums inside the backward plan; running statistics come out identical on every rank.
+        Otherwise (no group, or one rank) the plans are the plain ones, as SyncBatchNorm falls back to batch_norm."""
         self.model = model
         self.hyp = dict(HYP_FINETUNE_DOTA if hyp is None else hyp)
         nbs = 64
@@ -183,6 +189,8 @@ class TrainStep:
             broadcast_model_state(model, 0)
             if hasattr(model, "_bump_generation"):
                 model._bump_generation()
+        self.sync_bn = bool(sync_bn) and self.world > 1
+        model.bn_group = dist.group.WORLD if self.sync_bn else None
         freeze_layers(model, freeze)
         if not any(p.requires_grad for p in model.parameters()):
             raise RuntimeError(f"freeze={list(freeze)} freezes every parameter of the model: nothing is left to train")

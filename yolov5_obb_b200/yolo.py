@@ -216,7 +216,11 @@ class _TrainFn(torch.autograd.Function):
 
 class Model(nn.Module):
     """Drop-in for models/yolo.py:95 Model: Model(cfg, ch=3, nc=None, anchors=None); forward(x[B,3,H,W] in [0,1])
-    -> eval: (pred[B, sum(3*H_i*W_i), nc+185] fp32, None); train: list of nl (3, or 4 for P6) [B,3,H_i,W_i,nc+185] logits."""
+    -> eval: (pred[B, sum(3*H_i*W_i), nc+185] fp32, None); train: list of nl (3, or 4 for P6) [B,3,H_i,W_i,nc+185] logits.
+    bn_group: a torch.distributed process group makes every BatchNorm of the training plans a SyncBatchNorm over it
+    (train.py --sync-bn; set by TrainStep(sync_bn=True)); None: per-process batch statistics.  Never deep-copied."""
+
+    bn_group = None
 
     def __init__(self, cfg="yolov5s.yaml", ch=3, nc=None, anchors=None):
         super().__init__()
@@ -295,7 +299,7 @@ class Model(nn.Module):
         """copy.deepcopy(model) (ModelEMA, checkpoints): parameters and buffers are copied, the device plans are not."""
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
-        skip = ("_engines", "_last_train_engine", "_sig_tensors", "_sig_nbt", "_train_arena")
+        skip = ("_engines", "_last_train_engine", "_sig_tensors", "_sig_nbt", "_train_arena", "bn_group")
         new.__dict__ = {k: deepcopy(v, memo) for k, v in self.__dict__.items() if k not in skip}
         new._engines = {}
         new._sig_tensors = None
@@ -336,14 +340,17 @@ class Model(nn.Module):
                                "(val.py / detect.py --half); train the fp32 model and call .half() on a copy for inference")
         in_hw = (int(x.shape[2]), int(x.shape[3]))
         hw = in_hw if size is None else (int(size[0]), int(size[1]))
-        key = ("train", tuple(x.shape), x.device.index) + ((hw,) if hw != in_hw else ())
+        group = self.bn_group
+        key = ("train", tuple(x.shape), x.device.index) + ((hw,) if hw != in_hw else ()) + \
+            (("sync_bn", id(group)) if group is not None else ())
         eng = self._engines.get(key)
         refresh = eng is not None          # an existing plan re-packs the (possibly updated) parameters first
         if eng is None:
             arena = getattr(self, "_train_arena", None)
             if arena is not None and arena.device != x.device:
                 arena = None
-            eng = self._engines[key] = TrainEngine(self, x.shape[0], hw[0], hw[1], x.device, in_hw=in_hw, arena=arena)
+            eng = self._engines[key] = TrainEngine(self, x.shape[0], hw[0], hw[1], x.device, in_hw=in_hw, arena=arena,
+                                                   bn_group=group)
         eng._refresh_next = refresh
         self._last_train_engine = eng
         self._bump_generation()  # running statistics move (the captured graph bumps no version counter)
